@@ -1,13 +1,15 @@
 #!/usr/bin/env python
 """bench.py -- headline benchmark of the monai_b200 hot path (sliding-window inference, voxels/sec).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload unet_c2|swin_c3] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload unet_c2|swin_c3] [--impl b200|reference] [--dump-outputs DIR]
 
 One "step" = one full `SlidingWindowInferer(...)(volume, network)` pass over one synthetic volume.
   value : voxels/s with the volume already resident in HBM (CUDA-event timed, max over ranks)
   e2e   : the same call with a pinned HOST volume: H2D copy + inference + D2H copy of the logits inside the timed region
   roofline / cpu_baseline / clocks / gpu_launches : see DESIGN.md "Measurement"
 `--impl reference` times the reference algorithm's CPU path (the oracle port: torch-CPU restatement, all host threads).
+`--dump-outputs DIR` writes what the last timed step returned as float32 .npy files (a fixed, seeded sample of a large
+output), so that two builds can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -79,8 +81,9 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(hbm=d.get("hbm_gbs", 6650.0), tf=d.get("bf16_tflops", 1590.0), tf_sustained=d.get("bf16_tflops_sustained", 1400.0), src="measured")
-    return dict(hbm=6650.0, tf=1590.0, tf_sustained=1400.0, src="fallback")
+        return dict(hbm=d.get("hbm_gbs", 3350.0), tf=d.get("bf16_tflops", 989.0), tf_sustained=d.get("bf16_tflops_sustained", 989.0), src="measured")
+    # H100 SXM data sheet (dense fp16 / bf16, HBM3), for a card allowed 700 W; not reached in practice
+    return dict(hbm=3350.0, tf=989.0, tf_sustained=989.0, src="H100 SXM data sheet")
 
 
 def build_net(kind: str, device, half: bool):
@@ -102,7 +105,7 @@ def build_net(kind: str, device, half: bool):
 
 
 class ClockSampler:
-    """nvidia-smi sampling during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi sampling during the timed region."""
 
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -138,6 +141,28 @@ class ClockSampler:
                 if v.strip().lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": mx, "samples": len(sm), "reasons": sorted(reasons)}
+
+
+DUMP_VALUES = 12 << 20   # float32 values written in all (48 MB), shared equally by the dumped arrays
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Write each tensor as <out_dir>/<name>.npy in float32.  A tensor larger than its share of DUMP_VALUES is replaced by the
+    values at that many flat indices drawn with a fixed seed (the same for every run of the same shapes), and its float64
+    sum, absolute sum, minimum and maximum are written as <name>_stats.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_VALUES // max(1, len(arrays))
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > share:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randint(0, flat.numel(), (share,), generator=g).to(flat.device)
+            f64 = flat.double()
+            stats = torch.stack([f64.sum(), f64.abs().sum(), f64.min(), f64.max()])
+            np.save(os.path.join(out_dir, f"{name}_stats.npy"), stats.cpu().numpy())
+            del f64
+            flat = flat[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), flat.float().cpu().numpy())
 
 
 def run_reference(args, wl):
@@ -274,9 +299,15 @@ def run_transforms(args, wl):
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     out_host = None
 
+    last, keep = {}, bool(args.dump_outputs)
+
     def step_resident():
+        ys = []
         for v in dev_vols:
             y = pipe({"image": MetaTensor(v, affine=aff)})["image"]
+            if keep:
+                ys.append(y)
+        last["y"] = ys
         return y
 
     def step_e2e():
@@ -315,8 +346,12 @@ def run_transforms(args, wl):
     sampler = ClockSampler(local) if rank == 0 else None
     l0 = _lib.launch_count()
     ms_total = timed(step_resident, args.steps, args.warmup)
+    y_timed = last.pop("y")
     launches = (_lib.launch_count() - l0) * args.steps // (args.steps + args.warmup)
     clocks = sampler.stop() if sampler else {}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {f"image_{i:02d}": y for i, y in enumerate(y_timed)})
+    del y_timed
     ms_e2e = timed(step_e2e, args.steps, 1)
     K.profile_start()
     y = step_resident()
@@ -387,6 +422,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--sw-batch", type=int, default=0, help="override the workload's sw_batch_size")
     ap.add_argument("--no-secondary", action="store_true", help="skip the C2 / C4 lines appended to the default single-GPU run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned to DIR/<name>.npy (float32; large outputs as a seeded sample)")
     args = ap.parse_args()
     if os.environ.get("B200_BENCH_WATCHDOG"):
         import faulthandler
@@ -441,10 +478,12 @@ def main():
         from monai_b200.parallel import ShardedSlidingWindowInferer
 
         inferer = ShardedSlidingWindowInferer(wl["roi"], wl["sw_batch"], wl["overlap"], wl["mode"])
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
+    last = {}
 
     def step_resident():
-        return inferer(x_dev, net)
+        last["y"] = inferer(x_dev, net)
+        return last["y"]
 
     out_host = None
     if world > 1:
@@ -499,8 +538,12 @@ def main():
     sampler = ClockSampler(local) if rank == 0 else None
     l0 = _lib.launch_count()
     ms_total = timed(step_resident, args.steps, args.warmup)
+    y_timed = last.pop("y")
     launches = (_lib.launch_count() - l0) * args.steps // (args.steps + args.warmup)
     clocks = sampler.stop() if sampler else {}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"logits": y_timed})
+    del y_timed
     ms_e2e = timed(step_e2e, args.steps, 1)
 
     # per-kernel device time (CUDA events around every C-ABI launch, one extra untimed-for-value pass)

@@ -1,5 +1,5 @@
 /*
- * monai_b200 C ABI -- the drop-in boundary of the B200-native sliding-window / spatial-transform hot path.
+ * monai_b200 C ABI -- the drop-in boundary of the H100-native sliding-window / spatial-transform hot path.
  *
  * The reference (Project-MONAI/MONAI) has NO native boundary for this path: the seam is Python
  * (monai/inferers/utils.py, monai/networks/blocks/convolutions.py, monai/transforms/spatial/array.py), and
@@ -167,7 +167,7 @@ int b200_separable_filter3d(const void* src, int dtype, int C, int D, int H, int
                             const float* taps_h, int n_h, const float* taps_w, int n_w, float* tmp, void* dst,
                             void* stream);
 
-/* ---- tensor-core path (tcgen05 / TMEM / TMA), channel-blocked fp16 activations -------------------------- */
+/* ---- tensor-core path (wgmma / TMA), channel-blocked fp16 activations -------------------------- */
 /* Activation layout "NC8": [N][C/8][D][H][W][8] float16 (C % 8 == 0).  */
 
 /* NCDHW (f16/f32) <-> NC8 (f16) repack; c_off/Ctot address a channel slice of a concat buffer. */
@@ -176,7 +176,7 @@ int b200_unpack_nc8(const void* x, int Ctot, int c_off, int N, int C, long long 
 
 /* bytes needed for the packed weight image of b200_conv3x3x3_tc (depends on Cin, Cout only). */
 long long b200_conv3x3x3_tc_weight_bytes(int Cin, int Cout);
-/* pack Conv3d weight [Cout,Cin,3,3,3] float32 (device) into the UMMA B-operand image (device, fp16). */
+/* pack Conv3d weight [Cout,Cin,3,3,3] float32 (device) into the wgmma B-operand image (device, fp16). */
 int b200_conv3x3x3_tc_pack_weight(const float* w, int Cin, int Cout, void* packed, void* stream);
 
 typedef struct b200_conv_tc_desc {
@@ -202,9 +202,9 @@ typedef struct b200_conv_tc_desc {
   float* res_stats;
 } b200_conv_tc_desc;
 
-/* 3x3x3, stride 1, zero padding 1 implicit-GEMM convolution on tcgen05 tensor cores: halo tile staged once
- * into shared memory by TMA, 27 taps issued as shifted UMMA shared-memory descriptors, fp32 accumulators in
- * TMEM.  stats (optional, overwritten) receives per-(n,cout) {sum, sumsq} of the fp32 results so InstanceNorm needs no
+/* 3x3x3, stride 1, zero padding 1 implicit-GEMM convolution on wgmma tensor cores: halo tile staged once
+ * into shared memory by TMA, 27 taps issued as shifted wgmma shared-memory descriptors, fp32 accumulators in
+ * registers.  stats (optional, overwritten) receives per-(n,cout) {sum, sumsq} of the fp32 results so InstanceNorm needs no
  * extra pass.  The sums are DETERMINISTIC (bit-identical run to run): the epilogue warps write partial rows into
  * `workspace` (device scratch of b200_conv3x3x3_tc_workspace_bytes(desc) bytes, required when stats != NULL; no
  * initialisation needed) and a finishing pass adds them in a fixed order -- no floating-point atomics anywhere.
@@ -224,7 +224,7 @@ typedef struct b200_conv_gather_desc {
   int out_dtype;
 } b200_conv_gather_desc;
 
-/* General Conv3d / ConvTranspose3d (k <= 3, stride <= 2) as an implicit GEMM on tcgen05 with a cp.async im2col
+/* General Conv3d / ConvTranspose3d (k <= 3, stride <= 2) as an implicit GEMM on wgmma with a cp.async im2col
  * producer -- the stride-2 and transposed 3x3x3 layers of UNet (monai/networks/nets/unet.py:150-182).  Weights are
  * packed per (N tile, parity class, live tap, 16-channel slice); stats as in b200_conv3x3x3_tc. */
 long long b200_conv_gather_tc_weight_bytes(const b200_conv_gather_desc* desc);
@@ -252,10 +252,10 @@ typedef struct b200_gemm_tc_desc {
 } b200_gemm_tc_desc;
 
 long long b200_gemm_tc_weight_bytes(int N, int K);
-/* pack W[n,k] = w[n*stride_n + k*stride_k] (float32 device) into the UMMA B-operand image (fp16 device). */
+/* pack W[n,k] = w[n*stride_n + k*stride_k] (float32 device) into the wgmma B-operand image (fp16 device). */
 int b200_gemm_tc_pack_weight(const float* w, int N, int K, long long stride_n, long long stride_k, void* packed,
                              void* stream);
-/* y = [res +] act(x * W^T + bias) on tcgen05: nn.Linear (swin_unetr.py:509-532, blocks/mlp.py:75-80, PatchMerging
+/* y = [res +] act(x * W^T + bias) on wgmma: nn.Linear (swin_unetr.py:509-532, blocks/mlp.py:75-80, PatchMerging
  * 749-773), 1x1x1 Conv3d (dynunet_block.py:75-87) and ConvTranspose3d k2 s2 (unetr_block.py:56-64, mode 2 with
  * GEMM columns ordered [tap = kd*4+kh*2+kw][cout]).  stats (optional, overwritten) receives per-(batch, column)
  * {sum, sumsq} of the stored values for InstanceNorm, deterministically, through `workspace`
@@ -314,10 +314,10 @@ int b200_patch_merge_ln_nc8(const void* x, int N, int C, int D, int H, int W, co
 int b200_window_attention_nc8(const void* qkv, int N, int C, int heads, int nW, int n, float scale, const float* table,
                               int ws0, int ws1, int ws2, const int32_t* region, void* out, void* stream);
 
-/* The same attention on tcgen05 tensor cores (n <= 352 tokens per window, head_dim 16): S = q k^T and the
- * relative-position bias + shift mask are BOTH accumulated by tcgen05.mma (the bias as an fp16 B operand resident in
- * shared memory, multiplied by an identity held in TMEM), softmax reads the scores from TMEM, P V runs on tcgen05 with V
- * read in place (MN-major operand) and a ones column for the row sums.  Differences to b200_window_attention_nc8:
+/* The same attention on wgmma tensor cores (n <= 352 tokens per window, head_dim 16): S = q k^T and the
+ * relative-position bias + shift mask are BOTH accumulated by wgmma (the bias as an fp16 B operand resident in
+ * shared memory, multiplied by an identity held in shared memory), online softmax in registers, P V runs on wgmma with the
+ * probabilities as register operands and V read in place (MN-major operand).  Differences to b200_window_attention_nc8:
  *   - q must be PRE-SCALED by scale * log2(e) (fold it into the q rows of the qkv projection): scores are in log2 units;
  *   - the bias table and the shift mask are pre-packed per (mask type, head, 128-row tile) with
  *     b200_window_attention_tc_pack_bias: region_types int32 [ntypes][n] holds ONE representative row of `region` per
@@ -337,7 +337,7 @@ int b200_conv_cin1_nc8(const void* x, int dtype, int N, int D, int H, int W, con
                        int Cout, int k, int stride, int pad, void* y, int out_ctot, int out_coff, float* stats,
                        void* workspace, void* stream);
 
-/* The same on tcgen05 tensor cores for (k, stride, pad) = (3, 1, 1) and (2, 2, 0), Cout in {16, 32, 48, 64, 96, 128}: an
+/* The same on wgmma tensor cores for (k, stride, pad) = (3, 1, 1) and (2, 2, 0), Cout in {16, 32, 48, 64, 96, 128}: an
  * implicit GEMM with K = taps padded to 32 / 16 whose im2col operand is built in shared memory from a staged halo patch
  * of the raw volume; bound by the fp16 store of its output instead of by CUDA-core FMAs.  Same arguments. */
 long long b200_conv_cin1_tc_workspace_bytes(int N, int D, int H, int W, int Cout, int k, int stride, int pad);

@@ -1,4 +1,4 @@
-"""Build the in-tree CUDA library (sm_100a only) with nvcc; no torch extension machinery is involved.
+"""Build the in-tree CUDA library (sm_90a only) with nvcc; no torch extension machinery is involved.
 
 `python -m monai_b200._build` or `monai_b200._build.build()` compiles every `csrc/*.cu` into
 `monai_b200/lib/libmonai_b200.so` (cross-compiles without a GPU).  Objects are cached by source mtime.
@@ -18,7 +18,7 @@ OBJDIR = ROOT / "build"
 LIB = LIBDIR / "libmonai_b200.so"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I", str(ROOT.parent / "include"),
 ]
 
@@ -52,7 +52,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(_compile, srcs))
     if force or not LIB.exists() or any(o.stat().st_mtime > LIB.stat().st_mtime for o in objs):
-        cmd = [NVCC, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
+        cmd = [NVCC, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,7 +1,7 @@
 """Tensor-level wrappers around the C ABI (include/monai_b200.h).
 
 PyTorch only supplies device memory and the current stream here; every computation below is a hand-written
-sm_100a kernel reached through ctypes.  All functions require CUDA tensors.
+sm_90a kernel reached through ctypes.  All functions require CUDA tensors.
 """
 from __future__ import annotations
 
@@ -502,7 +502,7 @@ def channel_post(x: torch.Tensor, op: int, param: float = 0.0, onehot: int = 0, 
 
 # ---------------------------------------------------------------------------------------------- tensor-core path
 class NC8:
-    """fp16 activation buffer in the channel-blocked layout [N][C/8][D][H][W][8] used by the tcgen05 kernels."""
+    """fp16 activation buffer in the channel-blocked layout [N][C/8][D][H][W][8] used by the tensor-core kernels."""
 
     __slots__ = ("buf", "N", "C", "sp")
 
@@ -628,7 +628,7 @@ def cat_channels(tensors: Sequence[torch.Tensor]) -> torch.Tensor:
 
 
 def gemm_tc_pack_weight(w2d: torch.Tensor) -> torch.Tensor:
-    """Pack W[N,K] (any float dtype, device) into the UMMA B-operand image used by gemm_tc."""
+    """Pack W[N,K] (any float dtype, device) into the wgmma B-operand image used by gemm_tc."""
     L.require_cuda(w2d)
     w32 = w2d.detach().float().contiguous()
     N, Kd = w32.shape
@@ -764,7 +764,7 @@ def window_attention_tc_pack_bias(table: torch.Tensor, heads: int, n: int, windo
 
 
 def window_attention_tc(qkv: NC8, Cc: int, heads: int, nW: int, n: int, packed_bias: torch.Tensor, sched: torch.Tensor, ntypes: int) -> NC8:
-    """Window attention on tcgen05 (b200_window_attention_tc); q must be pre-scaled by scale * log2(e)."""
+    """Window attention on wgmma (b200_window_attention_tc); q must be pre-scaled by scale * log2(e)."""
     out = NC8(qkv.N, Cc, qkv.sp, qkv.buf.device)
     n_pad = (n + 31) // 32 * 32
     _call("window_attention_tc", L.ptr(qkv.buf), qkv.N, Cc, heads, nW, n, L.ptr(packed_bias), L.ptr(sched), ntypes, L.ptr(out.buf),
@@ -772,7 +772,7 @@ def window_attention_tc(qkv: NC8, Cc: int, heads: int, nW: int, n: int, packed_b
     return out
 
 
-ATTN_TC = not bool(os.environ.get("B200_ATTN_HMMA"))   # tcgen05 attention unless the mma.sync kernel is forced (debugging)
+ATTN_TC = not bool(os.environ.get("B200_ATTN_HMMA"))   # tensor-core attention unless the mma.sync kernel is forced (debugging)
 LOG2E = 1.4426950408889634
 
 

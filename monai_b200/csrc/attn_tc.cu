@@ -1,43 +1,27 @@
-// Windowed multi-head self-attention on tcgen05 tensor cores (SURVEY.md §8 row a13).
+// Windowed multi-head self-attention on Hopper wgmma tensor cores (SURVEY.md §8 row a13).
 //
 // Reference: WindowAttention.forward (monai/networks/nets/swin_unetr.py:509-532): per window of n <= 343 tokens and head
 // (head_dim 16):  softmax(q k^T * scale + relative_position_bias[:n,:n] + shift_mask) v.
 //
-// One persistent CTA per SM works on tiles = (window, head, 128-query row tile).  Per tile
-//   S[128 x n_pad] = Q K^T                      1 tcgen05.mma per key half   (SS form, K = 16 = the whole head)
-//                  + I[128 x 128] * B'          8 tcgen05.mma per key half   (TS form: A = identity held in TMEM)
+// One persistent CTA per SM works on tiles = (window, head, 128-query row tile); two consumer warpgroups take 64 query rows
+// each and walk the keys in blocks of 32 (flash-attention style, online softmax):
+//   S[64 x 32] = Q K^T                          1 wgmma (SS form, K = 16 = the whole head)
+//              + I[64 x 64] * B'                4 wgmma (A = the identity rows of the warpgroup, resident in shared memory)
 // where B'[i][j] = log2(e) * (bias[i][j] + mask[i][j]) is an fp16 B operand that stays RESIDENT in shared memory: it depends
 // on (head, row tile, mask type) only, so tiles are scheduled (mask type, head, row tile)-major and a CTA reloads it a
 // handful of times per launch.  Adding the bias with the tensor core (1.0 * fp16 value into the fp32 accumulator: exact)
-// removes the per-element table lookup and mask test that bounded the mma.sync kernel (swin.cu) -- with head_dim 16 the
-// tensor pipe is otherwise idle.  Padded keys carry B' = -30000 (P = 0).  Scores are in log2 units: the caller folds
-// scale * log2(e) into the q rows of the qkv projection.
-//   softmax: the two key halves of a tile are INDEPENDENT pipelines (flash-attention style): each half has its own exact row
-//            maximum m_h (pass 1 over TMEM), its own P_h = ex2(S_h - m_h) -- fp32 MUFU, packed to fp16 pairs and stored with
-//            tcgen05.st over the TMEM columns of S_h that the thread has already read (pass 2) -- and its own accumulator
-//   O_h[128 x 32] = P_h [V | 1 | 0]_h           n_pad/32 tcgen05.mma in TS form (A = P_h from TMEM), V read in place as an
-//            MN-major B operand (NC8 rows are 16-byte vectors of 8 dims); the ones column accumulates the row sums l_h in fp32;
-//   epilogue: O = (a0 O0 + a1 O1) / (a0 l0 + a1 l1), a_h = 2^(m_h - max(m0, m1))  -> fp16 NC8.
-// Because no maximum is shared between the halves, the tensor pipe computes PV_h(i) and S_h(i+1) for one half while the softmax
-// warps of the OTHER half exponentiate: TMEM has room for one S tile only (2 x 176 + 2 x 32 + 64 identity columns), and the
-// earlier single-maximum version (both halves needed before any exponential) left every softmax warp idle for the ~1 000 cycles
-// the S MMAs of the next tile take -- 8 300 cycles per tile against a MUFU floor of 2 816 (ncu: 33 % issue-active, MUFU 38 %,
-// tensor 25 %).
-// History of the P path (stage-1 shape, batch 8, ms; profiles/r02_attention_phase_db.jsonl, timelines read with
-// profiles/read_attn_trace.py from B200_ATTN_TRACE dumps): P through a shared-memory A image (SS MMAs, N = 32: bound by the 4 KB
-// A read, 59 cycles each) 0.473 -> P in TMEM (TS MMAs) 0.445 -> Q / K / V double-buffered in the 90 KB the P image freed
-// (the refill of the single buffers sat on the critical path of each half: softmax -> PV -> S) 0.418 -> S1 held half a period
-// behind S0 so that the exponential passes of the two halves do not share the MUFU 0.385 (shifted windows 0.533 -> 0.406).
+// removes the per-element table lookup and mask test.  Padded keys carry B' = -30000 (P = 0).  Scores are in log2 units:
+// the caller folds scale * log2(e) into the q rows of the qkv projection.
+//   softmax: running row maximum m and row sum l in registers; P = 2^(S - m) rounded to fp16 -- the S accumulator fragment
+//            of a 32-key block is, packed to fp16 pairs, the register A operand of two K = 16 steps of
+//   O[64 x 16] += P V                           2 wgmma (RS form), V read in place as an MN-major B operand (NC8 rows are
+//            16-byte vectors of 8 dims); l sums the same fp16-rounded P values the MMA consumes;
+//   epilogue: O / l -> fp16 NC8.
 // Q, K, V tiles are 1-D bulk copies of NC8 rows (contiguous per 8-channel chunk); the producer runs up to two tiles ahead.
 //
-// Warp roles (576 threads): warp 0 = copy producer, warp 1 = TMEM owner + MMA issuer, warps 2-9 = softmax of key half 0,
-// warps 10-17 = softmax of key half 1 (+ the epilogue); the two threads of a (query row, half) split its 16-column chunks and
-// exchange their maxima through shared memory and a 64-thread named barrier.
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
+// Warp roles (384 threads): warp 0 = copy producer, warps 4-7 / 8-11 = the two consumer warpgroups.
 #include "common.cuh"
-#include "tc05.cuh"
+#include "tc90.cuh"
 #include "../../include/monai_b200.h"
 
 namespace b200 {
@@ -46,17 +30,13 @@ constexpr int kAtNPadMax = 352;                       // keys per window, padded
 constexpr int kAtKChunk = kAtNPadMax * 16;            // bytes of one 8-dim chunk of K / V in shared memory
 constexpr int kAtBiasBytes = 16 * kAtNPadMax * 16;    // 16 chunks of 8 query rows
 constexpr int kAtIdBytes = 16 * 2048;                 // identity operand image: [k chunk of 8][128 rows][16 B]
-constexpr int kAtQBytes = 2 * 2048, kAtKBytes = 2 * kAtKChunk, kAtVBytes = 4 * kAtKChunk;   // one buffer of each (two of each are kept)
-constexpr int kAtColS1 = 176, kAtColO0 = 352, kAtColI = 384, kAtColO1 = 448;   // TMEM columns: S half 0 at 0, S half 1, O of half 0 (32), identity (64), O of half 1 (32)
-constexpr int kAtSmem = kAtBiasBytes + kAtIdBytes + 2 * (kAtQBytes + kAtKBytes + kAtVBytes) + 8 * 128 * 4 + 256 + 128;
+constexpr int kAtQBytes = 2 * 2048, kAtKBytes = 2 * kAtKChunk, kAtVBytes = 2 * kAtKChunk;   // one buffer of each (two of each are kept)
+constexpr int kAtSmem = kAtBiasBytes + kAtIdBytes + 2 * (kAtQBytes + kAtKBytes + kAtVBytes) + 2 * 2 * tc::kStageFloats * 4 + 256 + 128;
 constexpr float kAtPadBias = -30000.f;
-constexpr int kAtPhaseDefault = 175;                  // cycles per 32 padded keys (1 925 for 352 keys ~ half a tile period); see B200_ATTN_PHASE
 
 struct AttnTcParams {
   const __half* qkv; __half* out; const __half* bias; const int32_t* sched;
   int N, C8, heads, nW, n, n_pad, nrt, ntypes;
-  int phase_delay;      // cycles the S MMAs of key half 1 are held behind those of half 0 (0 = none): keeps the two softmax pipelines in anti-phase
-  long long* trace;     // debug timeline (B200_ATTN_TRACE): clock64 per (tile, role, event) of CTA 0, else null
 };
 
 struct AttnTile { int ty, h, rt, b, w; };
@@ -84,67 +64,49 @@ __device__ __forceinline__ AttnTile attn_decode(const AttnTcParams& p, long long
   return t;
 }
 
-// 2^(a - m), 2^(b - m) as packed fp16.  (ex2.approx.f16x2 is split by ptxas into one MUFU per half plus a PRMT, so the fp32
-// MUFU form costs the same MUFU slots, one instruction less, and keeps the exponent argument in fp32.)
-__device__ __forceinline__ uint32_t exp2_pack(float a, float b, float m) {
-  float ea, eb;
-  // volatile: keeps the exponentials BEHIND the tcgen05.ld of the next chunk in program order (the prefetch must be issued first)
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(ea) : "f"(a - m));
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(eb) : "f"(b - m));
-  const __half2 h = __floats2half2_rn(ea, eb);
+__device__ __forceinline__ float ex2(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
+// 2^(a - m), 2^(b - m) as packed fp16; `sum` accumulates the two ROUNDED values (what the PV MMA multiplies)
+__device__ __forceinline__ uint32_t exp2_pack(float a, float b, float m, float& sum) {
+  const __half2 h = __floats2half2_rn(ex2(a - m), ex2(b - m));
+  const float2 r = __half22float2(h);
+  sum += r.x + r.y;
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// running maximum of 16 fp32 TMEM values (FMNMX3: two values per instruction)
-__device__ __forceinline__ float max16(const uint32_t (&v)[16], float m) {
-#pragma unroll
-  for (int j = 0; j < 16; j += 2) asm("max.f32 %0, %0, %1, %2;" : "+f"(m) : "f"(__uint_as_float(v[j])), "f"(__uint_as_float(v[j + 1])));
-  return m;
-}
+constexpr int kAtThreads = 384;
 
-constexpr int kAtThreads = 64 + 512;        // producer, MMA issuer, 16 softmax warps (2 key halves x 2 threads per query row)
-
-template <int NPAD, bool TRACE = false>
+template <int NPAD>
 __global__ void __launch_bounds__(kAtThreads, 1) window_attention_tc_kernel(AttnTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = tc::align_smem128(smem_raw);   // keeps the shared address space (LDS/STS, not generic LD/ST)
   uint8_t* s_bias = smem;
-  uint8_t* s_id = s_bias + kAtBiasBytes;              // identity operand image, copied to TMEM once
+  uint8_t* s_id = s_bias + kAtBiasBytes;              // identity operand image
   uint8_t* s_q = s_id + kAtIdBytes;                   // [2 buffers][2 chunks][128 rows][16 B]
   uint8_t* s_k = s_q + 2 * kAtQBytes;                 // [2 buffers][2 chunks][n_pad keys][16 B]
-  uint8_t* s_v = s_k + 2 * kAtKBytes;                 // [2 buffers][4 chunk slots: V dims 0-7, 8-15, ones column, zeros]
-  float* s_max = reinterpret_cast<float*>(s_v + 2 * kAtVBytes);   // [half][sub][128]: maxima exchanged by the two threads of a (row, half)
-  float* s_hmax = s_max + 4 * 128;                                // [tile parity][half][128]: half maxima for the epilogue
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_hmax + 4 * 128);
+  uint8_t* s_v = s_k + 2 * kAtKBytes;                 // [2 buffers][2 chunks: V dims 0-7, 8-15][n_pad keys][16 B]
+  float* s_stage = reinterpret_cast<float*>(s_v + 2 * kAtVBytes);   // [2 warpgroups][2][kStageFloats]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + 2 * 2 * tc::kStageFloats);
   uint64_t* qk_full = bars + 0;     // [2]  Q / K (+ bias) of a tile have landed in buffer b
-  uint64_t* qk_empty = bars + 2;    // [2]  the S MMAs that read buffer b are done
+  uint64_t* qk_empty = bars + 2;    // [2]  the S MMAs that read buffer b are done (one arrival per consumer warpgroup)
   uint64_t* v_full = bars + 4;      // [2]
   uint64_t* v_empty = bars + 6;     // [2]  the PV MMAs that read V buffer b are done
-  uint64_t* s_full = bars + 8;      // [2]  per key half
-  uint64_t* s_empty = bars + 10;    // [2]
-  uint64_t* p_full = bars + 12;     // [2]
-  uint64_t* pv_done = bars + 14;    // [2]
-  uint64_t* o_empty = bars + 16;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 17);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  auto mark = [&](long long it, int role, int ev) {
-    if (TRACE && blockIdx.x == 0 && lane == 0 && it < 64) p.trace[(it * 3 + role) * 8 + ev] = clock64();
-  };
-  // NPAD (keys per window, padded to a multiple of 32) is a template parameter: the softmax passes are straight-line code
-  constexpr int n_pad = NPAD, NH = NPAD / 2;
-  constexpr int nchunk = NH / 16;                    // 16-key chunks of a half
-  constexpr int kCMax = (nchunk + 1) / 2;            // chunks of the larger of the two per-thread shares
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
+  // NPAD (keys per window, padded to a multiple of 32) is a template parameter: the key loop has a fixed trip count
+  constexpr int n_pad = NPAD;
   const int n = p.n;
   const long long T = (long long)p.nW * n;
   const long long total = (long long)p.N * p.nW * p.heads * p.nrt;
   const long long lo = total * blockIdx.x / gridDim.x, hi = total * (blockIdx.x + 1) / gridDim.x;
 
   if (threadIdx.x == 0) {
-    tc::mbar_init(o_empty, 4);
     for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&qk_full[i], 1); tc::mbar_init(&qk_empty[i], 1); tc::mbar_init(&v_full[i], 1); tc::mbar_init(&v_empty[i], 1);
-      tc::mbar_init(&s_full[i], 1); tc::mbar_init(&s_empty[i], 8); tc::mbar_init(&p_full[i], 8); tc::mbar_init(&pv_done[i], 1);
+      tc::mbar_init(&qk_full[i], 1); tc::mbar_init(&qk_empty[i], 2); tc::mbar_init(&v_full[i], 1); tc::mbar_init(&v_empty[i], 2);
     }
     tc::fence_barrier_init();
   }
@@ -157,19 +119,11 @@ __global__ void __launch_bounds__(kAtThreads, 1) window_attention_tc_kernel(Attn
   }
   __syncthreads();
   {
-    for (int j = threadIdx.x; j < 2 * kAtNPadMax; j += blockDim.x) {      // the ones column of both V buffers
-      __half* ones = reinterpret_cast<__half*>(s_v + (j / kAtNPadMax) * kAtVBytes + 2 * kAtKChunk);
-      ones[(j % kAtNPadMax) * 8] = __float2half_rn(1.f);
-    }
     __half* id = reinterpret_cast<__half*>(s_id);   // [k chunk of 8][row][8]: element (row r, k = r) = 1
     for (int r = threadIdx.x; r < 128; r += blockDim.x) id[((r >> 3) * 128 + r) * 8 + (r & 7)] = __float2half_rn(1.f);
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, 512);
   tc::fence_proxy_async();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ===================== copy producer: runs up to two tiles ahead of the MMAs =====================
@@ -205,235 +159,103 @@ __global__ void __launch_bounds__(kAtThreads, 1) window_attention_tc_kernel(Attn
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const bool leader = tc::elect_one();
-    const uint32_t tm = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const uint32_t idesc_s = tc::make_idesc_f16(128, NH);
-    const uint32_t idesc_pv = tc::make_idesc_f16(128, 32) | (1u << 16);   // B (= V) is MN-major
-    const uint32_t q_a = tc::smem_u32(s_q), k_a = tc::smem_u32(s_k), v_a = tc::smem_u32(s_v), b_a = tc::smem_u32(s_bias), i_a = tc::smem_u32(s_id);
-    // identity -> TMEM (8 K-steps of 16: 8 columns each)
-    if (leader)
-      for (int s = 0; s < 8; ++s) tc::tmem_cp_128x256b(tm + kAtColI + 8 * s, tc::make_desc_kmajor_noswz(i_a + s * 4096, 2048, 128));
-    __syncwarp();
-    // S = Q K^T + I B' for one key half of the tile whose Q / K sit in buffer b
-    auto issue_s = [&](int hf, int b) {
-      const uint32_t ts = tm + hf * kAtColS1;
-      const uint64_t qd = tc::make_desc_kmajor_noswz(q_a + b * kAtQBytes, 2048, 128);
-      const uint64_t kd = tc::make_desc_kmajor_noswz(k_a + b * kAtKBytes + hf * NH * 16, kAtKChunk, 128);
-      if (leader) tc::mma_f16_ss(ts, qd, kd, idesc_s, 0u);
-      for (int s = 0; s < 8; ++s) {
-        const uint64_t bd = tc::make_desc_kmajor_noswz(b_a + (2 * s) * n_pad * 16 + hf * NH * 16, n_pad * 16, 128);
-        if (leader) tc::mma_f16_ts(ts, tm + kAtColI + 8 * s, bd, idesc_s, 1u);
-      }
-      if (leader) tc::mma_commit(&s_full[hf]);
-      __syncwarp();
-    };
-    // O_hf = P_hf [V | 1 | 0]_hf: every key half has its own accumulator (its probabilities are scaled by its own row maximum).
-    // TS form: P (fp16 pairs) was stored over the S columns of its own half by the softmax threads -- chunk s sits at the start
-    // of the S range of the thread that wrote it (the thread with the larger share, sub 0 of half 0 / sub 1 of half 1, owns
-    // kCMax chunks).  With P in shared memory (SS form) the N = 32 MMA was bound by the 4 KB A read: 59 cycles against 39.
-    auto issue_pv = [&](int hf, int b) {
-      const uint32_t to = tm + (hf ? kAtColO1 : kAtColO0);
-      const int cnt0 = hf ? nchunk - kCMax : kCMax;
-      for (int s = 0; s < nchunk; ++s) {
-        const int ks = hf * nchunk + s;
-        // MN-major B: 8 keys x 16 B (8 dims) per core matrix, next 8 keys +128 B (LBO), next 8 dims +chunk (SBO)
-        const uint64_t vd = tc::make_desc_kmajor_noswz(v_a + b * kAtVBytes + ks * 256, 128, kAtKChunk);
-        const int pcol = s < cnt0 ? 8 * s : 16 * cnt0 + 8 * (s - cnt0);
-        if (leader) tc::mma_f16_ts(to, tm + hf * kAtColS1 + pcol, vd, idesc_pv, s != 0 ? 1u : 0u);
-      }
-      if (leader) tc::mma_commit(&pv_done[hf]);
-      __syncwarp();
-    };
-    // Ping-pong between the key halves, across tiles: the issue order is  PV0(i), S0(i+1), PV1(i), S1(i+1) -- while the softmax
-    // warps of one half exponentiate, the tensor pipe works for the other half.  The two halves are equal loops
-    // (softmax -> PV -> S -> softmax) that only meet on the MUFU; started back to back they stay ~1 100 cycles apart and their
-    // exponential passes overlap half of the time at half rate each, so S1 is held `phase_delay` cycles behind S0 (anti-phase).
-    // Measured alternatives that were NOT faster: issuing S0(i+1) before PV0(i); all sixteen softmax warps on one half at a time;
-    // part of the exponentials as an FMA-pipe polynomial (profiles/r02_attention_poly_ab.jsonl); L2 prefetch of the next rows.
-    long long t_s0 = 0;
-    auto hold_half1 = [&]() {
-      if (p.phase_delay > 0) while (clock64() - t_s0 < p.phase_delay) { }
-    };
-    const long long ntile = hi - lo;
-    if (ntile > 0) {
-      tc::mbar_wait(&qk_full[0], 0u);
-      tc::fence_after_sync();
-      t_s0 = clock64();
-      issue_s(0, 0);
-      hold_half1();
-      issue_s(1, 0);
-      if (leader) tc::mma_commit(&qk_empty[0]);
-      __syncwarp();
-    }
-    for (long long it = 0; it < ntile; ++it) {
-      const uint32_t ph = (uint32_t)(it & 1);
-      const int b = (int)(it & 1), nb = b ^ 1;
-      const bool more = it + 1 < ntile;
-      tc::mbar_wait(&v_full[b], (uint32_t)((it >> 1) & 1));
-      tc::mbar_wait(&p_full[0], ph);
-      tc::mbar_wait(o_empty, ph ^ 1);               // the epilogue has read O0 / O1 of the previous tile
-      tc::fence_after_sync();
-      mark(it, 0, 0);
-      issue_pv(0, b);
-      if (more) {
-        tc::mbar_wait(&qk_full[nb], (uint32_t)(((it + 1) >> 1) & 1));   // Q, K (and bias) of tile it+1 have landed
-        tc::mbar_wait(&s_empty[0], ph);             // the softmax threads of half 0 have read S0 of tile it
-        tc::fence_after_sync();
-        mark(it, 0, 1);
-        t_s0 = clock64();
-        issue_s(0, nb);
-        mark(it, 0, 2);
-      }
-      tc::mbar_wait(&p_full[1], ph);
-      tc::fence_after_sync();
-      mark(it, 0, 3);
-      issue_pv(1, b);
-      if (leader) tc::mma_commit(&v_empty[b]);
-      __syncwarp();
-      if (more) {
-        tc::mbar_wait(&s_empty[1], ph);
-        tc::fence_after_sync();
-        hold_half1();
-        mark(it, 0, 4);
-        issue_s(1, nb);
-        mark(it, 0, 5);
-        if (leader) tc::mma_commit(&qk_empty[nb]);
-        __syncwarp();
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== softmax + epilogue (warps 2..17) =====================
-    // Warps 2-9 own key half 0, warps 10-17 key half 1; the two threads of a (query row, half) split its 16-column chunks.
-    const int jj = (warp - 2) >> 2;
-    const int hf = jj >> 1, sub = jj & 1;
-    const int q = warp & 3;                   // TMEM lane quarter
-    const int row = q * 32 + lane;
-    // contiguous chunk ranges; the thread that also runs the epilogue (half 1 / sub 0) takes the smaller share
-    const bool big = (sub == 0) != (hf == 1);                     // sub 0 of half 0 and sub 1 of half 1 take the larger share
-    const int cnt = big ? kCMax : nchunk - kCMax;                 // warp-uniform
-    const int c_lo = sub ? nchunk - cnt : 0;
-    const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16);
-    const uint32_t ts = tlane + hf * kAtColS1 + c_lo * 16;        // this thread's first S column (and first P column)
-    const int bar_id = 1 + hf * 4 + q;
-    const bool tr = TRACE && sub == 0 && q == 2;
+  } else if (warp >= 4) {
+    // ===================== consumers: warpgroup g owns query rows 64 g .. 64 g + 63 of every tile =====================
+    const int g = (warp >> 2) - 1, wid = warp & 3;
+    const uint32_t q_a = tc::smem_u32(s_q), k_a = tc::smem_u32(s_k), v_a = tc::smem_u32(s_v), b_a = tc::smem_u32(s_bias),
+                   i_a = tc::smem_u32(s_id);
+    float* stage = s_stage + g * 2 * tc::kStageFloats;
+    int sl = 0;
     int it = 0;
     for (long long f = lo; f < hi; ++f, ++it) {
-      const uint32_t ph = (uint32_t)(it & 1);
-      // ---- pass 1: exact maximum of this key half of the row (two independent running maxima)
-      float m = -INFINITY, m2 = -INFINITY;
-      tc::mbar_wait(&s_full[hf], ph);
-      tc::fence_after_sync();
-      if (tr) mark(it, 1 + hf, 0);
-      {
-        uint32_t va[16], vb[16];
-        if (cnt > 0) tc::tmem_ld16(ts, va);
+      const int b = it & 1;
+      const uint32_t use = (uint32_t)((it >> 1) & 1);
+      float o[8];
 #pragma unroll
-        for (int k = 0; k < kCMax; k += 2) {
-          if (k < cnt) {
-            tc::tmem_ld_wait16(va);
-            if (k + 1 < cnt) tc::tmem_ld16(ts + (k + 1) * 16, vb);
-            m = max16(va, m);
-          }
-          if (k + 1 < kCMax && k + 1 < cnt) {
-            tc::tmem_ld_wait16(vb);
-            if (k + 2 < cnt) tc::tmem_ld16(ts + (k + 2) * 16, va);
-            m2 = max16(vb, m2);
-          }
+      for (int j = 0; j < 8; ++j) o[j] = 0.f;
+      float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // rows 16 wid + lane/4 and + 8 of the warpgroup
+      tc::mbar_wait(&qk_full[b], use);
+      tc::mbar_wait(&v_full[b], use);
+      const uint64_t qd = tc::make_desc_kmajor_noswz(q_a + b * kAtQBytes + g * 1024, 2048, 128);
+#pragma unroll 1
+      for (int kb = 0; kb < n_pad / 32; ++kb) {
+        // ---- S = Q K^T + I B' for 32 keys ----
+        float sc[16];
+        tc::wg_fence();
+        tc::Mma<32>::ss<0>(sc, qd, tc::make_desc_kmajor_noswz(k_a + b * kAtKBytes + kb * 32 * 16, kAtKChunk, 128), 0u);
+#pragma unroll
+        for (int s4 = 0; s4 < 4; ++s4) {
+          const int ks = 4 * g + s4;   // the identity rows of this warpgroup are non-zero in K steps 4g .. 4g+3 only
+          const uint64_t id_d = tc::make_desc_kmajor_noswz(i_a + ks * 4096 + g * 1024, 2048, 128);
+          const uint64_t bd = tc::make_desc_kmajor_noswz(b_a + (2 * ks) * n_pad * 16 + kb * 32 * 16, n_pad * 16, 128);
+          tc::Mma<32>::ss<0>(sc, id_d, bd, 1u);
         }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        tc::wg_fence_acc<16>(sc);
+        // ---- online softmax (the 4 lanes of a quad share a row) ----
+        float x0 = sc[0], x1 = sc[2];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          x0 = fmaxf(x0, fmaxf(sc[4 * i], sc[4 * i + 1]));
+          x1 = fmaxf(x1, fmaxf(sc[4 * i + 2], sc[4 * i + 3]));
+        }
+        x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 1)); x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 2));
+        x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 1)); x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 2));
+        const float n0 = fmaxf(m0, x0), n1 = fmaxf(m1, x1);
+        const float a0 = ex2(m0 - n0), a1 = ex2(m1 - n1);
+        m0 = n0; m1 = n1;
+        l0 *= a0; l1 *= a1;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) { o[4 * i] *= a0; o[4 * i + 1] *= a0; o[4 * i + 2] *= a1; o[4 * i + 3] *= a1; }
+        uint32_t pa[2][4];
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+          pa[kk][0] = exp2_pack(sc[8 * kk + 0], sc[8 * kk + 1], m0, l0);
+          pa[kk][1] = exp2_pack(sc[8 * kk + 2], sc[8 * kk + 3], m1, l1);
+          pa[kk][2] = exp2_pack(sc[8 * kk + 4], sc[8 * kk + 5], m0, l0);
+          pa[kk][3] = exp2_pack(sc[8 * kk + 6], sc[8 * kk + 7], m1, l1);
+        }
+        // ---- O += P V (MN-major B: 8 keys x 16 B (8 dims) per core matrix, next 8 keys +128 B (LBO), next 8 dims +chunk (SBO)) ----
+        tc::wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+          const uint64_t vd = tc::make_desc_kmajor_noswz(v_a + b * kAtVBytes + (2 * kb + kk) * 256, 128, kAtKChunk);
+          tc::Mma<16>::rs<1>(o, pa[kk], vd, 1u);
+        }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        tc::wg_fence_acc<8>(o);
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(pa[kk][j])::"memory");   // A registers stay live until the wait
       }
-      m = fmaxf(m, m2);
-      if (tr) mark(it, 1 + hf, 1);
-      s_max[(hf * 2 + sub) * 128 + row] = m;
-      asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");
-      m = fmaxf(m, s_max[(hf * 2 + (sub ^ 1)) * 128 + row]);
-      if (sub == 0) s_hmax[((it & 1) * 2 + hf) * 128 + row] = m;     // read by the epilogue of this tile
-      if (tr) mark(it, 1 + hf, 2);
-      // ---- pass 2: P = 2^(S - m) as fp16 pairs, stored over the S columns this thread has already read: chunk k (8 columns)
-      //      lands inside S chunk k / 2 of the same thread, so neither the partner thread nor the load in flight is touched
-      {
-        uint32_t va[16], vb[16];
-        auto emit = [&](const uint32_t (&v)[16], int k) {
-          const uint32_t u0 = exp2_pack(__uint_as_float(v[0]), __uint_as_float(v[1]), m);
-          const uint32_t u1 = exp2_pack(__uint_as_float(v[2]), __uint_as_float(v[3]), m);
-          const uint32_t u2 = exp2_pack(__uint_as_float(v[4]), __uint_as_float(v[5]), m);
-          const uint32_t u3 = exp2_pack(__uint_as_float(v[6]), __uint_as_float(v[7]), m);
-          const uint32_t u4 = exp2_pack(__uint_as_float(v[8]), __uint_as_float(v[9]), m);
-          const uint32_t u5 = exp2_pack(__uint_as_float(v[10]), __uint_as_float(v[11]), m);
-          const uint32_t u6 = exp2_pack(__uint_as_float(v[12]), __uint_as_float(v[13]), m);
-          const uint32_t u7 = exp2_pack(__uint_as_float(v[14]), __uint_as_float(v[15]), m);
-          tc::tmem_st8(ts + 8 * k, u0, u1, u2, u3, u4, u5, u6, u7);
-        };
-        if (cnt > 0) tc::tmem_ld16(ts, va);
+      if (wid == 0 && lane == 0) { tc::mbar_arrive(&qk_empty[b]); tc::mbar_arrive(&v_empty[b]); }
+      // ---- epilogue: O / l -> fp16 NC8 (one row and 8 dims per thread after the slice exchange) ----
+      l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+      l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+      const float i0 = 1.f / l0, i1 = 1.f / l1;
 #pragma unroll
-        for (int k = 0; k < kCMax; k += 2) {
-          if (k < cnt) {
-            tc::tmem_ld_wait16(va);
-            if (k + 1 < cnt) tc::tmem_ld16(ts + (k + 1) * 16, vb);
-            emit(va, k);
-          }
-          if (k + 1 < kCMax && k + 1 < cnt) {
-            tc::tmem_ld_wait16(vb);
-            if (k + 2 < cnt) tc::tmem_ld16(ts + (k + 2) * 16, va);
-            emit(vb, k + 1);
-          }
-        }
-      }
-      if (tr) mark(it, 1 + hf, 4);
-      tc::tmem_st_wait();            // P has landed in TMEM
-      tc::fence_before_sync();       // ... and this thread's TMEM reads of this S half are complete
-      __syncwarp();                  // one arrival per warp (the barriers count 8): per-thread arrivals serialise on one word
-      if (lane == 0) { tc::mbar_arrive(&p_full[hf]); tc::mbar_arrive(&s_empty[hf]); }
-      if (hf == 1 && sub == 0) {
-        // ---- epilogue: combine the two halves (flash-attention style) and normalise:  O = (a0 O0 + a1 O1) / (a0 l0 + a1 l1),
-        //      a_h = 2^(m_h - max(m0, m1)), l_h = the ones column of O_h
-        const AttnTile t = attn_decode(p, f);
-        tc::mbar_wait(&pv_done[0], ph);
-        tc::mbar_wait(&pv_done[1], ph);
-        tc::fence_after_sync();
-        if (tr) mark(it, 2, 5);
-        uint32_t o0[16], o1[16], l0[8], l1[8];
-        tc::tmem_ld16(tlane + kAtColO0, o0);
-        tc::tmem_ld8(tlane + kAtColO0 + 16, l0);
-        tc::tmem_ld16(tlane + kAtColO1, o1);
-        tc::tmem_ld8(tlane + kAtColO1 + 16, l1);
-        const float m0 = s_hmax[((it & 1) * 2 + 0) * 128 + row], m1 = m;
-        tc::tmem_ld_wait();
-        tc::fence_before_sync();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(o_empty);
-        const int r = t.rt * 128 + row;
-        if (r < n) {
-          const float mm = fmaxf(m0, m1);
-          float a0, a1;
-          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(a0) : "f"(m0 - mm));
-          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(a1) : "f"(m1 - mm));
-          const float inv = 1.f / (a0 * __uint_as_float(l0[0]) + a1 * __uint_as_float(l1[0]));
-          a0 *= inv; a1 *= inv;
-          __half* ob = p.out + (long long)t.b * p.C8 * T * 8 + ((long long)t.w * n + r) * 8;
+      for (int i = 0; i < 2; ++i) { o[4 * i] *= i0; o[4 * i + 1] *= i0; o[4 * i + 2] *= i1; o[4 * i + 3] *= i1; }
+      float* buf = stage + (sl & 1) * tc::kStageFloats;
+      ++sl;
+      tc::wg_stage16<0>(o, buf, wid, lane);
+      tc::wg_bar(8 + g);
+      float v[8];
+      tc::wg_read8(buf, wid, lane, v);
+      const AttnTile t = attn_decode(p, f);
+      const int r = t.rt * 128 + 64 * g + 32 * (wid & 1) + lane;
+      if (r < n) {
+        const int dt = wid >> 1;
+        __half* ob = p.out + (long long)t.b * p.C8 * T * 8 + ((long long)t.w * n + r) * 8;
+        uint4 hv;
+        __half2* hp = reinterpret_cast<__half2*>(&hv);
 #pragma unroll
-          for (int dt = 0; dt < 2; ++dt) {
-            uint4 hv;
-            __half2* hp = reinterpret_cast<__half2*>(&hv);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int k = dt * 8 + 2 * j;
-              hp[j] = __floats2half2_rn(a0 * __uint_as_float(o0[k]) + a1 * __uint_as_float(o1[k]),
-                                        a0 * __uint_as_float(o0[k + 1]) + a1 * __uint_as_float(o1[k + 1]));
-            }
-            *reinterpret_cast<uint4*>(ob + (long long)(2 * t.h + dt) * T * 8) = hv;
-          }
-        }
-        if (tr) mark(it, 2, 6);
+        for (int j = 0; j < 4; ++j) hp[j] = __floats2half2_rn(v[2 * j], v[2 * j + 1]);
+        *reinterpret_cast<uint4*>(ob + (long long)(2 * t.h + dt) * T * 8) = hv;
       }
     }
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -516,26 +338,6 @@ extern "C" int b200_window_attention_tc(const void* qkv, int N, int C, int heads
   B200_REQUIRE(kern != nullptr, "window_attention_tc: no kernel for %d padded keys", p.n_pad);
   // per-device attribute: set on every call (cheap), so a second GPU in the same process works
   B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kAtSmem));
-  p.trace = nullptr;
-  // B200_ATTN_PHASE: cycles per 32 keys by which the S MMAs of key half 1 trail those of half 0 (see the MMA issuer)
-  static const int phase_q = [] { const char* e = std::getenv("B200_ATTN_PHASE"); return e ? std::atoi(e) : kAtPhaseDefault; }();
-  p.phase_delay = phase_q * (p.n_pad / 32);
-  // debug: B200_ATTN_TRACE=<file> records the phase timeline of CTA 0 of every n_pad = 352 launch (last launch wins)
-  static const char* trace_path = std::getenv("B200_ATTN_TRACE");
-  if (trace_path && p.n_pad == 352) {
-    static long long* trace_buf = nullptr;
-    if (!trace_buf) B200_CUDA(cudaMalloc(&trace_buf, 64 * 3 * 8 * sizeof(long long)));
-    B200_CUDA(cudaMemsetAsync(trace_buf, 0, 64 * 3 * 8 * sizeof(long long), (cudaStream_t)stream));
-    p.trace = trace_buf;
-    kern = window_attention_tc_kernel<352, true>;
-    B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kAtSmem));
-    kern<<<grid, kAtThreads, kAtSmem, (cudaStream_t)stream>>>(p);
-    B200_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    std::vector<long long> host(64 * 3 * 8);
-    B200_CUDA(cudaMemcpy(host.data(), trace_buf, host.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-    if (FILE* fp = std::fopen(trace_path, "wb")) { std::fwrite(host.data(), sizeof(long long), host.size(), fp); std::fclose(fp); }
-    return B200_OK;
-  }
   kern<<<grid, kAtThreads, kAtSmem, (cudaStream_t)stream>>>(p);
   B200_LAUNCH_CHECK("window_attention_tc_kernel");
   return B200_OK;

@@ -9,7 +9,7 @@
 // never materialised.  imp() is evaluated on the fly from the three 1-D
 // vectors of compute_importance_map (monai/data/utils.py:1084-1134): ((g_d*g_h)*g_w) clamped from below.
 #include "common.cuh"
-#include "tc05.cuh"
+#include "tc90.cuh"
 #include "blend.cuh"
 #include <cstdlib>
 #include "../../include/monai_b200.h"

@@ -1,4 +1,4 @@
-// Shared helpers for the monai_b200 CUDA kernels (sm_100a only).
+// Shared helpers for the monai_b200 CUDA kernels (sm_90a only).
 // Nothing here depends on torch; the C-ABI in include/monai_b200.h is plain pointers + sizes.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// Single-input-channel convolutions on tcgen05 tensor cores (SURVEY.md §8 rows a8, a12, a14).
+// Single-input-channel convolutions on Hopper wgmma tensor cores (SURVEY.md §8 rows a8, a12, a14).
 //
 // Replaces, for a ONE-channel fp16/fp32 input volume,
 //   * the 3x3x3 / stride 1 / pad 1 stem of UnetrBasicBlock.conv1 (monai/networks/blocks/dynunet_block.py:57-74), and
@@ -8,25 +8,20 @@
 //   M = 128 output voxels (a 16 x 8 patch of one D-plane, BD planes per tile), N = Cout, K = taps (zero padded),
 // so the kernel is bound by the fp16 NC8 store of its output (2 * Cout bytes per voxel) instead.
 //
-// Warp roles (160 + 128 * EG threads, EG = Cout / 16 epilogue groups, one persistent CTA per SM):
+// Warp roles (384 threads, one persistent CTA per SM):
 //   warps 0-3  producers: stage the raw halo patch of a tile in shared memory (plain loads, zero outside the volume
 //              = the convolution's zero padding), then build the im2col A operand -- thread r owns GEMM row r and
-//              writes its K-vector as 16-byte pieces straight into the UMMA K-major / no-swizzle core-matrix image
+//              writes its K-vector as 16-byte pieces straight into the wgmma K-major / no-swizzle core-matrix image
 //              ([k-chunk of 8][row][8 taps], LBO = 2048 B, SBO = 128 B); fence.proxy.async + mbarrier hand-over;
-//   warp 4     TMEM owner + MMA issuer (converged warp, one elected lane): BD x K/16 tcgen05.mma per tile;
-//   warps 5..  epilogue (conv_epi.cuh: conv_epilogue_cg), groups of four warps that each own fixed 8-channel chunks: bias,
-//              deterministic InstanceNorm sums kept in registers across tiles, NC8 store.
+//   warps 4-11 two consumer warpgroups (rows 0-63 / 64-127 of the tile): BD x K/16 wgmma per tile with the accumulators in
+//              registers, then the epilogue of conv_epi.cuh (bias, deterministic InstanceNorm sums, NC8 store).
 // The weights [Cout][taps] fp32 are packed into the B image in shared memory once per CTA.
 #include "common.cuh"
-#include "tc05.cuh"
+#include "tc90.cuh"
 #include "conv_epi.cuh"
 #include "../../include/monai_b200.h"
 
 namespace b200 {
-
-// epilogue warp groups: each owns a fixed set of 8-channel chunks (two per group up to Cout = 96) of every plane, see
-// conv_epilogue_cg -- per-channel sums stay in registers across tiles
-__host__ __device__ constexpr int cin1_eg(int NT) { return NT / 16 <= 6 ? (NT / 16 > 0 ? NT / 16 : 1) : 4; }
 
 template <int KS, int STRIDE, int NT, int BD>
 struct Cin1Cfg {
@@ -41,13 +36,11 @@ struct Cin1Cfg {
   static constexpr int kAStage = BD * kAPlane;
   static constexpr int kStages = 2;
   static constexpr int kBBytes = NT * kKP * 2;
-  static constexpr int kAccCols = 2 * BD * NT;
-  static constexpr int kTmemCols = (kAccCols <= 32) ? 32 : (kAccCols <= 64) ? 64 : (kAccCols <= 128) ? 128 : (kAccCols <= 256) ? 256 : 512;
-  static constexpr int kEG = cin1_eg(NT);
-  static constexpr int kThreads = 160 + 128 * kEG;
-  static constexpr int kSmemBytes = kStages * (kAStage + kHaloBytes) + kBBytes + 256 + kEG * 4 * 2 * NT * 4 + 128;
-  static_assert(kAccCols <= 512, "accumulators exceed TMEM");
-  static_assert(NT % 16 == 0 && NT >= 16 && NT <= 256, "invalid UMMA N");
+  static constexpr int kThreads = 384;                           // producer warpgroup + two consumer warpgroups
+  static constexpr int kSmemBytes = kStages * (kAStage + kHaloBytes) + kBBytes + 256 + 4 * 2 * NT * 4 +
+                                    2 * 2 * tc::kStageFloats * 4 + 128;
+  static_assert(BD * NT <= 256, "accumulators exceed the register budget of a consumer thread");
+  static_assert(NT % 16 == 0 && NT >= 16 && NT <= 256, "invalid wgmma N");
   static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
 };
 
@@ -72,21 +65,16 @@ __global__ void __launch_bounds__(Cin1Cfg<KS, STRIDE, NT, BD>::kThreads, 1) conv
   uint8_t* smem_b = smem_h + Cfg::kStages * Cfg::kHaloBytes;     // packed weights
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + Cfg::kBBytes);
   uint64_t* a_full = bars;               // [2], 128 producer arrivals
-  uint64_t* a_empty = bars + 2;          // [2], tcgen05.commit
-  uint64_t* acc_full = bars + 4;         // [2]
-  uint64_t* acc_empty = bars + 6;        // [2], one arrival per epilogue warp
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* a_empty = bars + 2;          // [2], one arrival per consumer warpgroup
   float* s_stats = reinterpret_cast<float*>(bars + 32);          // [4][2*NT]
+  float* s_stage = s_stats + 4 * 2 * NT;                         // [2 warpgroups][2][kStageFloats]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&a_full[i], 128); tc::mbar_init(&a_empty[i], 1);
-      tc::mbar_init(&acc_full[i], 1); tc::mbar_init(&acc_empty[i], 4 * Cfg::kEG);
-    }
+    for (int i = 0; i < 2; ++i) { tc::mbar_init(&a_full[i], 128); tc::mbar_init(&a_empty[i], 2); }
     tc::fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < Cfg::kEG * 4 * 2 * NT; i += blockDim.x) s_stats[i] = 0.f;
+  for (int i = threadIdx.x; i < 4 * 2 * NT; i += blockDim.x) s_stats[i] = 0.f;
   // B image [k16][khalf][NT/8][8 cout][8 k] (same as gemm_tc): element (cout, k) with k = (kd*KS + kh)*KS + kw
   {
     __half* sb = reinterpret_cast<__half*>(smem_b);
@@ -102,12 +90,8 @@ __global__ void __launch_bounds__(Cin1Cfg<KS, STRIDE, NT, BD>::kThreads, 1) conv
       sb[i] = __float2half_rn(k < Cfg::kTaps ? p.w[cout * Cfg::kTaps + k] : 0.f);
     }
   }
-  if (warp == 4) tc::tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc::fence_proxy_async();     // the generic-proxy writes of the weight image must be visible to tcgen05.mma
-  tc::fence_before_sync();
+  tc::fence_proxy_async();     // the generic-proxy writes of the weight image must be visible to the wgmma operand reads
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 4) {
     // ===================== producers: halo patch -> im2col A image =====================
@@ -166,42 +150,39 @@ __global__ void __launch_bounds__(Cin1Cfg<KS, STRIDE, NT, BD>::kThreads, 1) conv
       tc::fence_proxy_async();
       tc::mbar_arrive(&a_full[st]);
     }
-  } else if (warp == 4) {
-    // ===================== MMA issuer =====================
-    const bool leader = tc::elect_one();
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const uint32_t idesc = tc::make_idesc_f16(128, NT);
+  } else {
+    // ===================== consumers: BD x K/16 wgmma per tile, then the epilogue of their 64 rows =====================
+    const int g = (warp >> 2) - 1, wid = warp & 3;
+    float* stage = s_stage + g * 2 * tc::kStageFloats;
+    float* ws = s_stats + (2 * g + (wid & 1)) * (2 * NT);
     const uint32_t b_base = tc::smem_u32(smem_b);
-    int it = 0;
+    long long group = -1;
+    int sl = 0, it = 0;
     for (long long t = blockIdx.x; t < p.e.total_tiles; t += gridDim.x, ++it) {
       const int st = it & 1;
       const uint32_t ph = (uint32_t)((it >> 1) & 1);
-      tc::mbar_wait(&acc_empty[st], ph ^ 1);       // accumulator set st (it alternates with the A stage) has been drained
+      const ConvTile c = conv_tile<BD>(p.e, t);
+      float acc[BD * NT / 2];
       tc::mbar_wait(&a_full[st], ph);
-      tc::fence_after_sync();
-      const uint32_t a_base = tc::smem_u32(smem_a + st * Cfg::kAStage);
-      const uint32_t tacc = tmem_u + st * (BD * NT);
-#pragma unroll
-      for (int pl = 0; pl < BD; ++pl) {
+      const uint32_t a_base = tc::smem_u32(smem_a + st * Cfg::kAStage) + g * 1024;
+      tc::wg_fence();
+      tc::static_for<0, BD>([&](auto plc) {
+        constexpr int pl = decltype(plc)::value;
 #pragma unroll
         for (int ks = 0; ks < Cfg::kKP / 16; ++ks) {
           const uint64_t adesc = tc::make_desc_kmajor_noswz(a_base + pl * Cfg::kAPlane + ks * 4096, 2048, 128);
           const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_base + ks * NT * 32, NT * 16, 128);
-          if (leader) tc::mma_f16_ss(tacc + pl * NT, adesc, bdesc, idesc, ks != 0 ? 1u : 0u);
+          tc::wg_mma_ss<NT>(acc + pl * NT / 2, adesc, bdesc, ks != 0 ? 1u : 0u, 128);
         }
-      }
-      if (leader) { tc::mma_commit(&a_empty[st]); tc::mma_commit(&acc_full[st]); }
-      __syncwarp();
+      });
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc<BD * NT / 2>(acc);
+      if (wid == 0 && lane == 0) tc::mbar_arrive(&a_empty[st]);
+      conv_stats_turn(p.e, ws, NT, t, group, g, wid, lane);
+      conv_epilogue<NT, BD>(p.e, c, acc, stage, ws, g, wid, lane, sl);
     }
-    __syncwarp();
-  } else {
-    // ===================== epilogue (warps 5 .. 4 + 4 * kEG): group g takes its channel chunks of every plane =====================
-    conv_epilogue_cg<NT, BD, 2, Cfg::kEG>(p.e, tmem_base, acc_full, acc_empty, s_stats, warp, lane, (warp - 5) >> 2);
-  }
-  __syncthreads();
-  if (warp == 4) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, Cfg::kTmemCols);
+    conv_stats_final(p.e, ws, NT, group, g, wid, lane);
   }
 }
 
@@ -219,10 +200,10 @@ static int launch_cin1_tc(int N, int D, int H, int W, int pad, int out_ctot, int
   e.total_tiles = (long long)e.tiles_w * e.tiles_h * e.tiles_d * N;
   const long long sp_tiles = (long long)e.tiles_w * e.tiles_h * e.tiles_d;
   const int R = stats_rows(sp_tiles, e.total_tiles);
-  c.ws_bytes = stats_partial_bytes(N, R, NT, 4 * Cfg::kEG);
+  c.ws_bytes = stats_partial_bytes(N, R, NT, 4);
   if (c.query) return B200_OK;
   e.y = (__half*)c.y; e.bias = c.bias;
-  e.sp.buf = c.stats ? (float*)c.ws : nullptr; e.sp.R = R; e.sp.tiles_per_group = sp_tiles; e.sp.rows_per_cta = 4 * Cfg::kEG;
+  e.sp.buf = c.stats ? (float*)c.ws : nullptr; e.sp.R = R; e.sp.tiles_per_group = sp_tiles; e.sp.rows_per_cta = 4;
   dim3 grid((unsigned)std::min<long long>(e.total_tiles, num_sms()));
   if (c.dtype == B200_DT_F16) {
     auto kern = conv_cin1_tc_kernel<__half, KS, STRIDE, NT, BD>;
@@ -234,7 +215,7 @@ static int launch_cin1_tc(int N, int D, int H, int W, int pad, int out_ctot, int
     kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, c.st>>>(p);
   }
   B200_LAUNCH_CHECK("conv_cin1_tc_kernel");
-  if (c.stats) return launch_stats_finish((const float*)c.ws, N, R * 4 * Cfg::kEG, NT, 1, NT, c.stats, c.st);
+  if (c.stats) return launch_stats_finish((const float*)c.ws, N, R * 4, NT, 1, NT, c.stats, c.st);
   return B200_OK;
 }
 

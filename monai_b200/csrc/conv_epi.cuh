@@ -1,13 +1,13 @@
-// Shared output stage of the tcgen05 convolution kernels (conv_tc.cu: 3x3x3 stride 1; conv_cin1_tc.cu: the
-// single-input-channel stems): tile geometry and the TMEM -> registers -> fp16 NC8 epilogue with bias and the
+// Shared output stage of the wgmma convolution kernels (conv_tc.cu: 3x3x3 stride 1; conv_cin1_tc.cu: the
+// single-input-channel stems): tile geometry and the registers -> fp16 NC8 epilogue with bias and the
 // deterministic InstanceNorm partial sums of stats.cuh.
 //
 // GEMM rows of a tile = one 16 (H) x 8 (W) patch of an output D-plane; a tile holds BD consecutive planes whose fp32
-// accumulators are adjacent TMEM column blocks of NT columns; NB accumulator sets alternate between tiles.
+// accumulators are adjacent column blocks of NT columns in the registers of the two consumer warpgroups.
 #pragma once
 #include "common.cuh"
 #include "stats.cuh"
-#include "tc05.cuh"
+#include "tc90.cuh"
 
 namespace b200 {
 
@@ -37,295 +37,79 @@ __device__ __forceinline__ ConvTile conv_tile(const ConvEpiP& p, long long t) {
   return c;
 }
 
-// Run by EG groups of four epilogue warps (each group: four warps whose ids cover the residues mod 4 -- warp w reads TMEM lanes
-// 32*(w & 3) ..); group `eg` handles the planes sub = eg, eg + EG, ... of every tile.  acc_full[b] is completed by tcgen05.commit
-// of the MMA warp, acc_empty[b] expects 4 * EG arrivals (one per epilogue warp).  s_stats: shared memory, 4 * EG warp-private rows of 2*NT floats,
-// zero-initialised by the caller.  (One group suffices while the MMAs of a tile take longer than its epilogue -- conv_tc.cu; the
-// store-bound stems of conv_cin1_tc.cu run four groups.)
-template <int NT, int BD, int NB, int EG = 1>
-__device__ __forceinline__ void conv_epilogue(const ConvEpiP& p, uint32_t tmem_base, uint64_t* acc_full, uint64_t* acc_empty,
-                                              float* s_stats, int warp, int lane, int eg = 0) {
-  static_assert(BD % EG == 0 || EG == 1, "planes must divide evenly among the epilogue groups");
-  constexpr int kSubs = (BD + EG - 1) / EG;   // planes per group
-  const int q = warp & 3;                 // TMEM lane quarter this warp may access
+// Epilogue of one tile, run by the consumer warpgroup `g` (rows 64 g .. 64 g + 63 of the tile) from its wgmma accumulators:
+// `acc` holds the BD planes of the tile as consecutive blocks of NT columns (m64nN fragment layout, NT / 2 registers per
+// plane).  16-column slices pass through the warpgroup's two slice buffers `stage` (tc::wg_stage16); afterwards warp `wid`
+// owns row 32 (wid & 1) + lane of its half tile and the 8-column chunk 2 c16 + (wid >> 1) of every slice: + bias, fp16 NC8
+// store, and the running InstanceNorm sums of the chunk in the quarter's shared-memory row `ws` (the two warps of a quarter
+// own disjoint columns of the row).  `sl` counts slices across calls so the two buffers strictly alternate.
+template <int NT, int BD>
+__device__ __forceinline__ void conv_epilogue(const ConvEpiP& p, const ConvTile& c, const float* acc, float* stage, float* ws,
+                                              int g, int wid, int lane, int& sl) {
+  const int q = 2 * g + (wid & 1), half = wid >> 1;
   const int row = q * 32 + lane;
-  const int slot = eg * 4 + q;
   const long long S = (long long)p.D * p.H * p.W;
-  const long long sp_tiles = (long long)p.tiles_w * p.tiles_h * p.tiles_d;
-  float* ws = s_stats + slot * (2 * NT);
-  long long group = -1;
-  int it = 0;
-  for (long long t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++it) {
-    const ConvTile c = conv_tile<BD>(p, t);
+  const int h = c.h0 + (row >> 3), w = c.w0 + (row & 7);
+  const bool hw_ok = h < p.H && w < p.W;
+  const int co0 = c.nt * NT;
+  __half* ybase = p.y + (((long long)c.n * (p.out_ctot / 8) + (p.out_coff + co0) / 8) * S) * 8;
+#pragma unroll
+  for (int c16 = 0; c16 < NT / 16; ++c16) {
+    const int cc = 2 * c16 + half;
+    float bsum[8], bsq[8], bias8[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { bsum[j] = 0.f; bsq[j] = 0.f; bias8[j] = p.bias ? p.bias[co0 + cc * 8 + j] : 0.f; }
+#pragma unroll
+    for (int sub = 0; sub < BD; ++sub, ++sl) {
+      float* buf = stage + (sl & 1) * tc::kStageFloats;
+      tc::wg_stage16<0>(acc + (sub * NT + c16 * 16) / 2, buf, wid, lane);
+      tc::wg_bar(8 + g);
+      float f[8];
+      tc::wg_read8(buf, wid, lane, f);
+      const int dz = c.d0 + sub;
+      const bool ok = hw_ok && dz < p.D;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        f[j] += bias8[j];
+        if (ok) { bsum[j] += f[j]; bsq[j] = fmaf(f[j], f[j], bsq[j]); }
+      }
+      if (ok) {
+        uint4 hv;
+        __half2* hp = reinterpret_cast<__half2*>(&hv);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) hp[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
+        *reinterpret_cast<uint4*>(ybase + ((long long)cc * S + ((long long)dz * p.H + h) * p.W + w) * 8) = hv;
+      }
+    }
     if (p.sp.buf) {
-      const long long g = t / sp_tiles;
-      if (g != group) {
-        if (group >= 0) stats_flush(p.sp, ws, 2 * NT, group, slot, lane, 0, NT);
-        group = g;
+      float a1, b1;
+      transpose_reduce8(bsum, bsq, lane, a1, b1);
+      if ((lane & 3) == 0) {   // eight lanes, eight different columns of the quarter's row: no atomics
+        const int col = cc * 8 + transpose_reduce8_col(lane);
+        ws[2 * col] += a1;
+        ws[2 * col + 1] += b1;
       }
     }
-    const int buf = it % NB;
-    const uint32_t aph = (uint32_t)((it / NB) & 1);
-    const int h = c.h0 + (row >> 3), w = c.w0 + (row & 7);
-    const bool hw_ok = h < p.H && w < p.W;
-    const int co0 = c.nt * NT;
-    __half* ybase = p.y + (((long long)c.n * (p.out_ctot / 8) + (p.out_coff + co0) / 8) * S) * 8;
-    tc::mbar_wait(&acc_full[buf], aph);
-    tc::fence_after_sync();
-    const uint32_t tq = tmem_base + buf * (BD * NT) + ((uint32_t)(q * 32) << 16);
-    uint32_t vn[8];
-    tc::tmem_ld8(tq + eg * NT, vn);   // (cc = 0, first plane of this group); every later load is prefetched one step ahead
-#pragma unroll 1
-    for (int cc = 0; cc < NT / 8; ++cc) {
-      float bsum[8], bsq[8], bias8[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { bsum[j] = 0.f; bsq[j] = 0.f; bias8[j] = p.bias ? p.bias[co0 + cc * 8 + j] : 0.f; }
-#pragma unroll
-      for (int si = 0; si < kSubs; ++si) {
-        const int sub = eg + si * EG;
-        uint32_t v[8];
-        tc::tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = vn[j];
-        {
-          const int nsub = si + 1 < kSubs ? sub + EG : eg, ncc = si + 1 < kSubs ? cc : cc + 1;
-          if (ncc < NT / 8) tc::tmem_ld8(tq + nsub * NT + ncc * 8, vn);
-        }
-        const int dz = c.d0 + sub;
-        const bool ok = hw_ok && dz < p.D;
-        float f[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          f[j] = __uint_as_float(v[j]) + bias8[j];
-          if (ok) { bsum[j] += f[j]; bsq[j] = fmaf(f[j], f[j], bsq[j]); }
-        }
-        if (ok) {
-          uint4 hv;
-          __half2* hp = reinterpret_cast<__half2*>(&hv);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) hp[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-          *reinterpret_cast<uint4*>(ybase + ((long long)cc * S + ((long long)dz * p.H + h) * p.W + w) * 8) = hv;
-        }
-      }
-      if (p.sp.buf) {
-        float a1, b1;
-        transpose_reduce8(bsum, bsq, lane, a1, b1);
-        if ((lane & 3) == 0) {   // eight lanes, eight different columns of the warp-private row: no atomics
-          const int col = cc * 8 + transpose_reduce8_col(lane);
-          ws[2 * col] += a1;
-          ws[2 * col + 1] += b1;
-        }
-      }
-    }
-    // this thread's TMEM reads of the set are complete: hand it back to the MMA warp (one arrival per warp)
-    tc::fence_before_sync();
-    __syncwarp();
-    if (lane == 0) tc::mbar_arrive(&acc_empty[buf]);
-  }
-  if (p.sp.buf && group >= 0) stats_flush(p.sp, ws, 2 * NT, group, slot, lane, 0, NT);
-}
-
-// Two-output variant for conv3x3x3_tc with the folded 1x1x1 residual branch (conv_tc.cu, RES): the accumulator set holds the BD
-// planes of the 3x3x3 result at columns [0, BD*NT) and the BD planes of the 1x1x1 result at [BD*NT, 2*BD*NT).  `p` describes the main
-// output, `r` the residual output (its own tensor and statistics partials; no bias).
-// At NT = 48, BD = 4 only ONE accumulator set fits in TMEM, so the epilogue is on the critical path; two measures shorten it:
-//   * EG = 2 groups of four warps split the planes (group eg drains planes eg, eg + 2, ...);
-//   * the MAIN block is drained first and handed back through acc_empty -- the next tile's 3x3x3 MMAs only write the main block
-//     until the residual MMAs at the end of its first K slice -- then the residual block is drained and handed back through
-//     res_empty, which the MMA warp waits on right before those residual MMAs.
-// s_stats: 2 x 4 * EG warp-private rows of 2*NT floats (main rows first).  Both barriers expect 4 * EG arrivals (one per warp).
-template <int NT, int BD, int NB, int EG>
-__device__ __forceinline__ void conv_epilogue_res(const ConvEpiP& p, const ConvEpiP& r, uint32_t tmem_base, uint64_t* acc_full,
-                                                  uint64_t* acc_empty, uint64_t* res_empty, float* s_stats, int warp, int lane, int eg) {
-  constexpr int kSubs = (BD + EG - 1) / EG;
-  const int q = warp & 3;
-  const int row = q * 32 + lane;
-  const int slot = eg * 4 + q;
-  const long long S = (long long)p.D * p.H * p.W;
-  const long long sp_tiles = (long long)p.tiles_w * p.tiles_h * p.tiles_d;
-  float* ws_m = s_stats + slot * (2 * NT);
-  float* ws_r = s_stats + (4 * EG + slot) * (2 * NT);
-  long long group = -1;
-  int it = 0;
-  for (long long t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++it) {
-    const ConvTile c = conv_tile<BD>(p, t);
-    const long long g = t / sp_tiles;
-    if (g != group) {
-      if (group >= 0) {
-        if (p.sp.buf) stats_flush(p.sp, ws_m, 2 * NT, group, slot, lane, 0, NT);
-        if (r.sp.buf) stats_flush(r.sp, ws_r, 2 * NT, group, slot, lane, 0, NT);
-      }
-      group = g;
-    }
-    const int buf = it % NB;
-    const uint32_t aph = (uint32_t)((it / NB) & 1);
-    const int h = c.h0 + (row >> 3), w = c.w0 + (row & 7);
-    const bool hw_ok = h < p.H && w < p.W;
-    const int co0 = c.nt * NT;
-    tc::mbar_wait(&acc_full[buf], aph);
-    tc::fence_after_sync();
-    const uint32_t tq0 = tmem_base + buf * (2 * BD * NT) + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int which = 0; which < 2; ++which) {
-      const ConvEpiP& o = which ? r : p;
-      float* ws = which ? ws_r : ws_m;
-      const uint32_t tq = tq0 + which * (BD * NT);
-      __half* ybase = o.y + (((long long)c.n * (o.out_ctot / 8) + (o.out_coff + co0) / 8) * S) * 8;
-      uint32_t vn[8];
-      tc::tmem_ld8(tq + eg * NT, vn);
-#pragma unroll 1
-      for (int cc = 0; cc < NT / 8; ++cc) {
-        float bsum[8], bsq[8], bias8[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { bsum[j] = 0.f; bsq[j] = 0.f; bias8[j] = o.bias ? o.bias[co0 + cc * 8 + j] : 0.f; }
-#pragma unroll
-        for (int si = 0; si < kSubs; ++si) {
-          const int sub = eg + si * EG;
-          uint32_t v[8];
-          tc::tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] = vn[j];
-          {
-            const int nsub = si + 1 < kSubs ? sub + EG : eg, ncc = si + 1 < kSubs ? cc : cc + 1;
-            if (ncc < NT / 8 && nsub < BD) tc::tmem_ld8(tq + nsub * NT + ncc * 8, vn);
-          }
-          const int dz = c.d0 + sub;
-          const bool ok = hw_ok && sub < BD && dz < p.D;
-          float f[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            f[j] = __uint_as_float(v[j]) + bias8[j];
-            if (ok) { bsum[j] += f[j]; bsq[j] = fmaf(f[j], f[j], bsq[j]); }
-          }
-          if (ok) {
-            uint4 hv;
-            __half2* hp = reinterpret_cast<__half2*>(&hv);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) hp[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-            *reinterpret_cast<uint4*>(ybase + ((long long)cc * S + ((long long)dz * p.H + h) * p.W + w) * 8) = hv;
-          }
-        }
-        if (o.sp.buf) {
-          float a1, b1;
-          transpose_reduce8(bsum, bsq, lane, a1, b1);
-          if ((lane & 3) == 0) {
-            const int col = cc * 8 + transpose_reduce8_col(lane);
-            ws[2 * col] += a1;
-            ws[2 * col + 1] += b1;
-          }
-        }
-      }
-      // this block of the set is drained: hand it back (one arrival per warp)
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(which ? &res_empty[buf] : &acc_empty[buf]);
-    }
-  }
-  if (group >= 0) {
-    if (p.sp.buf) stats_flush(p.sp, ws_m, 2 * NT, group, slot, lane, 0, NT);
-    if (r.sp.buf) stats_flush(r.sp, ws_r, 2 * NT, group, slot, lane, 0, NT);
   }
 }
 
-// Channel-grouped variant for the store-bound stems (conv_cin1_tc.cu).  EG groups of four epilogue warps; group `eg` owns the
-// 8-channel chunks cc = eg, eg + EG, ... of EVERY plane of every tile, so a thread meets the same channels tile after tile and
-// keeps their InstanceNorm sums in REGISTERS: the cross-lane transpose-reduce (64 of the ~100 instructions a (row, chunk) cost
-// in conv_epilogue -- ncu: FSEL + FADD + SHFL = 40 % of the stem's instruction stream, issue-bound at 74 %) runs once per batch
-// item instead of once per (tile, plane, chunk).  The order of the additions is fixed (tile order), so the sums stay
-// deterministic.  acc_empty expects 4 * EG arrivals (one per warp); s_stats holds 4 * EG zero-initialised rows of 2 * NT floats.
-template <int NT, int BD, int NB, int EG>
-__device__ __forceinline__ void conv_epilogue_cg(const ConvEpiP& p, uint32_t tmem_base, uint64_t* acc_full, uint64_t* acc_empty,
-                                                 float* s_stats, int warp, int lane, int eg) {
-  constexpr int kChunks = NT / 8;
-  constexpr int kCC = (kChunks + EG - 1) / EG;   // chunks per group (the last groups may own one fewer)
-  const int q = warp & 3;
-  const int row = q * 32 + lane;
-  const int slot = eg * 4 + q;
-  const long long S = (long long)p.D * p.H * p.W;
-  const long long sp_tiles = (long long)p.tiles_w * p.tiles_h * p.tiles_d;
-  float* ws = s_stats + slot * (2 * NT);
-  float asum[kCC][8], asq[kCC][8];
-#pragma unroll
-  for (int ci = 0; ci < kCC; ++ci)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { asum[ci][j] = 0.f; asq[ci][j] = 0.f; }
-  auto flush = [&](long long group) {
-#pragma unroll
-    for (int ci = 0; ci < kCC; ++ci) {
-      const int cc = eg + ci * EG;
-      if (cc < kChunks) {
-        float a1, b1;
-        transpose_reduce8(asum[ci], asq[ci], lane, a1, b1);
-        if ((lane & 3) == 0) {
-          const int col = cc * 8 + transpose_reduce8_col(lane);
-          ws[2 * col] = a1;
-          ws[2 * col + 1] = b1;
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { asum[ci][j] = 0.f; asq[ci][j] = 0.f; }
-      }
-    }
-    stats_flush(p.sp, ws, 2 * NT, group, slot, lane, 0, NT);   // columns of other groups are zero in this row
-  };
-  long long group = -1;
-  int it = 0;
-  for (long long t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++it) {
-    const ConvTile c = conv_tile<BD>(p, t);
-    if (p.sp.buf) {
-      const long long g = t / sp_tiles;
-      if (g != group) {
-        if (group >= 0) flush(group);
-        group = g;
-      }
-    }
-    const int buf = it % NB;
-    const uint32_t aph = (uint32_t)((it / NB) & 1);
-    const int h = c.h0 + (row >> 3), w = c.w0 + (row & 7);
-    const bool hw_ok = h < p.H && w < p.W;
-    __half* ybase = p.y + (((long long)c.n * (p.out_ctot / 8) + p.out_coff / 8) * S + ((long long)c.d0 * p.H + h) * p.W + w) * 8;
-    tc::mbar_wait(&acc_full[buf], aph);
-    tc::fence_after_sync();
-    const uint32_t tq = tmem_base + buf * (BD * NT) + ((uint32_t)(q * 32) << 16) + eg * 8;
-    uint32_t vn[8];
-    tc::tmem_ld8(tq, vn);   // (chunk 0, plane 0) of this group; every later load is prefetched one step ahead
-#pragma unroll
-    for (int ci = 0; ci < kCC; ++ci) {
-      const int cc = eg + ci * EG;
-      if (cc < kChunks) {
-        float bias8[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) bias8[j] = p.bias ? p.bias[cc * 8 + j] : 0.f;
-#pragma unroll
-        for (int sub = 0; sub < BD; ++sub) {
-          uint32_t v[8];
-          tc::tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] = vn[j];
-          {
-            const int nsub = sub + 1 < BD ? sub + 1 : 0, nci = sub + 1 < BD ? ci : ci + 1;
-            if (nci < kCC && eg + nci * EG < kChunks) tc::tmem_ld8(tq + nsub * NT + nci * EG * 8, vn);
-          }
-          const bool ok = hw_ok && c.d0 + sub < p.D;
-          if (ok) {
-            uint4 hv;
-            __half2* hp = reinterpret_cast<__half2*>(&hv);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float f0 = __uint_as_float(v[2 * j]) + bias8[2 * j], f1 = __uint_as_float(v[2 * j + 1]) + bias8[2 * j + 1];
-              asum[ci][2 * j] += f0; asq[ci][2 * j] = fmaf(f0, f0, asq[ci][2 * j]);
-              asum[ci][2 * j + 1] += f1; asq[ci][2 * j + 1] = fmaf(f1, f1, asq[ci][2 * j + 1]);
-              hp[j] = __floats2half2_rn(f0, f1);
-            }
-            *reinterpret_cast<uint4*>(ybase + ((long long)cc * S + (long long)sub * p.H * p.W) * 8) = hv;
-          }
-        }
-      }
-    }
-    tc::fence_before_sync();
-    __syncwarp();
-    if (lane == 0) tc::mbar_arrive(&acc_empty[buf]);
+// Statistics bookkeeping before the epilogue of tile t: when the (batch item, N tile) group changes, the quarter's row of
+// running sums is written to the partial buffer (slot = quarter; rows_per_cta = 4) by the first warp of the quarter, after
+// the warpgroup barrier has made the other warp's sums visible.
+__device__ __forceinline__ void conv_stats_turn(const ConvEpiP& p, float* ws, int NT, long long t, long long& group, int g, int wid,
+                                                int lane) {
+  const long long g_t = t / ((long long)p.tiles_w * p.tiles_h * p.tiles_d);
+  if (g_t == group) return;
+  if (group >= 0 && p.sp.buf) {
+    tc::wg_bar(8 + g);
+    if ((wid >> 1) == 0) stats_flush(p.sp, ws, 2 * NT, group, 2 * g + (wid & 1), lane, 0, NT);
   }
-  if (p.sp.buf && group >= 0) flush(group);
+  group = g_t;
+}
+__device__ __forceinline__ void conv_stats_final(const ConvEpiP& p, float* ws, int NT, long long group, int g, int wid, int lane) {
+  if (group < 0 || !p.sp.buf) return;
+  tc::wg_bar(8 + g);
+  if ((wid >> 1) == 0) stats_flush(p.sp, ws, 2 * NT, group, 2 * g + (wid & 1), lane, 0, NT);
 }
 
 }  // namespace b200

@@ -1,4 +1,4 @@
-// General 3-D convolution / transposed convolution (kernel <= 3, any stride) as an implicit GEMM on tcgen05 tensor
+// General 3-D convolution / transposed convolution (kernel <= 3, any stride) as an implicit GEMM on Hopper wgmma tensor
 // cores with a software im2col producer (SURVEY.md §8 row a8: the stride-2 Conv3d and ConvTranspose3d(k3, s2) layers
 // of UNet, monai/networks/nets/unet.py:150-182 via monai/networks/blocks/convolutions.py:131-152).
 //
@@ -6,13 +6,13 @@
 // stride s: s^3 classes, so that every row of a tile uses the same set of live taps -- no work is spent on taps that
 // cannot reach an output voxel), columns = NT output channels, K = (live taps) x Cin walked in units of 16 channels.
 // Producer warps (128 threads, one GEMM row each) gather the 16-channel vectors of the tap's input voxel with
-// cp.async (16-byte pieces of the NC8 layout, zero-filled outside the volume = zero padding) straight into the UMMA
-// K-major / no-swizzle core-matrix image; a proxy fence + mbarrier hands each stage to the single-thread MMA issuer.
-// Weights are pre-packed per (N tile, class, tap, 16-channel slice) and arrive by bulk copies.  The kernel is
-// persistent with two TMEM accumulator buffers; 4 epilogue warps add bias, reduce InstanceNorm partial sums and store
-// either NC8 fp16 (optionally into a channel slice of a concat buffer) or NCDHW (the Cout = 2 segmentation head).
+// cp.async (16-byte pieces of the NC8 layout, zero-filled outside the volume = zero padding) straight into the wgmma
+// K-major / no-swizzle core-matrix image; a proxy fence + mbarrier hands each stage to the two consumer warpgroups
+// (rows 0-63 / 64-127 of the tile, accumulators in registers).  Weights are pre-packed per (N tile, class, tap,
+// 16-channel slice) and arrive by bulk copies.  The kernel is persistent; the consumers' epilogue adds bias, reduces
+// InstanceNorm partial sums and stores either NC8 fp16 (optionally into a channel slice of a concat buffer) or NCDHW (the Cout = 2 segmentation head).
 #include "common.cuh"
-#include "tc05.cuh"
+#include "tc90.cuh"
 #include "stats.cuh"
 #include "../../include/monai_b200.h"
 
@@ -28,7 +28,7 @@ struct CgParams {
   b200_conv_gather_desc d;
   const __half* x; const __half* w; const float* bias; void* y;
   StatsPartials sp;           // deterministic InstanceNorm partial sums (stats.cuh)
-  int NT, tmem_cols, cout_pad;
+  int NT, cout_pad;
   int ncls, mul;              // classes; input coordinate = coarse * mul + tap offset
   int Dc, Hc, Wc;             // coarse extent of one class
   int cls_ntaps[8], cls_unit_off[8];
@@ -98,23 +98,21 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int sr
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
 
-__global__ void __launch_bounds__(288, 1) conv_gather_tc_kernel(CgParams p) {
+template <int NT>
+__global__ void __launch_bounds__(384, 1) conv_gather_tc_kernel(CgParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = tc::align_smem128(smem_raw);   // keeps the shared address space (LDS/STS, not generic LD/ST)
-  const int NT = p.NT;
-  const int b_stage = kCgUnits * NT * 32;
+  constexpr int b_stage = kCgUnits * NT * 32;
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kCgStages * kCgAStage;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + kCgStages * b_stage);
   uint64_t* full = bars;                         // producers (128) + weight copy (1 + tx)
-  uint64_t* empty = bars + kCgStages;
-  uint64_t* acc_full = bars + 2 * kCgStages;     // [2]
-  uint64_t* acc_empty = acc_full + 2;            // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_stats = reinterpret_cast<float*>(bars + 16);
+  uint64_t* empty = bars + kCgStages;            // one arrival per consumer warpgroup
+  float* s_stats = reinterpret_cast<float*>(bars + 16);   // [4][2*NT]
+  float* s_stage = s_stats + 4 * 2 * NT;                  // [2 warpgroups][2][kStageFloats]
 
   const b200_conv_gather_desc& d = p.d;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int kcs = d.Cin / 16;
   const int n_tiles = p.cout_pad / NT;
   const long long coarse = (long long)p.Dc * p.Hc * p.Wc;
@@ -123,23 +121,18 @@ __global__ void __launch_bounds__(288, 1) conv_gather_tc_kernel(CgParams p) {
   const long long Si = (long long)d.Di * d.Hi * d.Wi, So = (long long)d.Do * d.Ho * d.Wo;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kCgStages; ++i) { tc::mbar_init(&full[i], 129); tc::mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&acc_full[i], 1); tc::mbar_init(&acc_empty[i], 128); }
+    for (int i = 0; i < kCgStages; ++i) { tc::mbar_init(&full[i], 129); tc::mbar_init(&empty[i], 2); }
     tc::fence_barrier_init();
   }
   for (int i = threadIdx.x; i < 4 * 2 * NT; i += blockDim.x) s_stats[i] = 0.f;
-  if (warp == 4) tc::tmem_alloc(tmem_slot, p.tmem_cols);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 4) {
     // ===================== im2col producers: thread r gathers GEMM row r =====================
     const int r = threadIdx.x;
     int s = 0; uint32_t ph = 0;
     // up to kCgInflight cp.async groups (= stages) stay in flight per thread; a stage is handed to the MMA warp only
-    // after its group completed (wait_group) and a proxy fence made the generic-proxy writes visible to tcgen05
+    // after its group completed (wait_group) and a proxy fence made the generic-proxy writes visible to wgmma
     constexpr int kCgInflight = 3;
     int pend_first = 0, pend_n = 0;   // pending stages are pend_first, pend_first+1, ... (mod kCgStages)
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -192,54 +185,24 @@ __global__ void __launch_bounds__(288, 1) conv_gather_tc_kernel(CgParams p) {
       tc::fence_proxy_async();
       for (; pend_n > 0; --pend_n) { tc::mbar_arrive(&full[pend_first]); pend_first = (pend_first + 1) % kCgStages; }
     }
-  } else if (warp == 4) {
-    // ===================== MMA issuer =====================
-    // converged warp + one elected lane (see conv_tc.cu): descriptors stay on the uniform datapath
-    {
-      const bool leader = tc::elect_one();
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-      const uint32_t idesc = tc::make_idesc_f16(128, NT);
-      int s = 0; uint32_t ph = 0;
-      int it = 0;
-      for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-        const int cls = (int)((tile / row_tiles) % p.ncls);
-        const int units = p.cls_ntaps[cls] * kcs;
-        const int buf = it & 1;
-        const uint32_t aph = (uint32_t)((it >> 1) & 1);
-        tc::mbar_wait(&acc_empty[buf], aph ^ 1);
-        tc::fence_after_sync();
-        const uint32_t tacc = tmem_u + buf * NT;
-        for (int u0 = 0; u0 < units; u0 += kCgUnits) {
-          const int nu = min(kCgUnits, units - u0);
-          tc::mbar_wait(&full[s], ph);
-          tc::fence_after_sync();
-          const uint32_t a_base = tc::smem_u32(smem_a + s * kCgAStage), b_base = tc::smem_u32(smem_b + s * b_stage);
-          for (int q = 0; q < nu; ++q) {
-            const uint64_t adesc = tc::make_desc_kmajor_noswz(a_base + q * 2 * 2048, 2048, 128);
-            const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_base + q * NT * 32, NT * 16, 128);
-            if (leader) tc::mma_f16_ss(tacc, adesc, bdesc, idesc, (u0 | q) != 0 ? 1u : 0u);
-          }
-          if (leader) tc::mma_commit(&empty[s]);
-          __syncwarp();
-          if (++s == kCgStages) { s = 0; ph ^= 1; }
-        }
-        if (leader) tc::mma_commit(&acc_full[buf]);
-        __syncwarp();
-      }
-    }
-    __syncwarp();
   } else {
-    // ===================== epilogue (warps 5..8) =====================
-    const int q = warp & 3;
+    // ===================== consumers: warpgroup g runs rows 64 g .. 64 g + 63 (wgmma, then the epilogue) =====================
+    const int g = (warp >> 2) - 1, wid = warp & 3;
+    const int q = 2 * g + (wid & 1), half = wid >> 1;
     float* ws = s_stats + q * (2 * NT);
+    float* stage = s_stage + g * 2 * tc::kStageFloats;
     long long group = -1;
-    int it = 0;
-    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+    int s = 0; uint32_t ph = 0;
+    int sl = 0;
+    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       if (p.sp.buf) {
-        const long long g = tile / ((long long)p.ncls * row_tiles);
-        if (g != group) {
-          if (group >= 0) stats_flush(p.sp, ws, 2 * NT, group, q, lane, 0, NT);
-          group = g;
+        const long long gg = tile / ((long long)p.ncls * row_tiles);
+        if (gg != group) {
+          if (group >= 0) {
+            tc::wg_bar(8 + g);
+            if (half == 0) stats_flush(p.sp, ws, 2 * NT, group, q, lane, 0, NT);
+          }
+          group = gg;
         }
       }
       // tile order: row tile fastest, then parity class, then N tile, then batch item (consecutive tiles share their
@@ -249,8 +212,24 @@ __global__ void __launch_bounds__(288, 1) conv_gather_tc_kernel(CgParams p) {
       const int cls = (int)(t2 % p.ncls); t2 /= p.ncls;
       const int nt = (int)(t2 % n_tiles);
       const int n = (int)(t2 / n_tiles);
-      const int buf = it & 1;
-      const uint32_t aph = (uint32_t)((it >> 1) & 1);
+      const int units = p.cls_ntaps[cls] * kcs;
+      float acc[NT / 2];
+      for (int u0 = 0; u0 < units; u0 += kCgUnits) {
+        const int nu = min(kCgUnits, units - u0);
+        tc::mbar_wait(&full[s], ph);
+        const uint32_t a_base = tc::smem_u32(smem_a + s * kCgAStage) + g * 1024, b_base = tc::smem_u32(smem_b + s * b_stage);
+        tc::wg_fence();
+        for (int qq = 0; qq < nu; ++qq) {
+          const uint64_t adesc = tc::make_desc_kmajor_noswz(a_base + qq * 2 * 2048, 2048, 128);
+          const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_base + qq * NT * 32, NT * 16, 128);
+          tc::wg_mma_ss<NT>(acc, adesc, bdesc, (u0 | qq) != 0 ? 1u : 0u, 128);
+        }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        tc::wg_fence_acc<NT / 2>(acc);
+        if (wid == 0 && lane == 0) tc::mbar_arrive(&empty[s]);
+        if (++s == kCgStages) { s = 0; ph ^= 1; }
+      }
       const long long cv = (long long)rt * 128 + q * 32 + lane;
       bool ok = cv < coarse;
       long long orow = 0;
@@ -264,22 +243,17 @@ __global__ void __launch_bounds__(288, 1) conv_gather_tc_kernel(CgParams p) {
         orow = ((long long)oz * d.Ho + oy) * d.Wo + ox;
       }
       const int co0 = nt * NT;
-      tc::mbar_wait(&acc_full[buf], aph);
-      tc::fence_after_sync();
-      const uint32_t tacc = tmem_base + buf * NT + ((uint32_t)(q * 32) << 16);
-      uint32_t vn[8];
-      tc::tmem_ld8(tacc, vn);
-#pragma unroll 1
-      for (int cc = 0; cc < NT / 8; ++cc) {
-        uint32_t v[8];
-        tc::tmem_ld_wait();
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = vn[j];
-        if (cc + 1 < NT / 8) tc::tmem_ld8(tacc + (cc + 1) * 8, vn);
-        const int nc = co0 + cc * 8;
+      for (int c16 = 0; c16 < NT / 16; ++c16, ++sl) {
+        float* buf = stage + (sl & 1) * tc::kStageFloats;
+        tc::wg_stage16<0>(acc + c16 * 8, buf, wid, lane);
+        tc::wg_bar(8 + g);
         float f[8];
+        tc::wg_read8(buf, wid, lane, f);
+        const int cc = 2 * c16 + half;
+        const int nc = co0 + cc * 8;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[j]) + ((p.bias && nc + j < d.Cout) ? p.bias[nc + j] : 0.f);
+        for (int j = 0; j < 8; ++j) f[j] += (p.bias && nc + j < d.Cout) ? p.bias[nc + j] : 0.f;
         if (ok) {
           if (d.out_layout == 0) {
             if (nc < d.Cout) {
@@ -303,31 +277,40 @@ __global__ void __launch_bounds__(288, 1) conv_gather_tc_kernel(CgParams p) {
           float a8[8], b8[8];
 #pragma unroll
           for (int j = 0; j < 8; ++j) { a8[j] = ok ? f[j] : 0.f; b8[j] = a8[j] * a8[j]; }
-          float cs, cq;
-          transpose_reduce8(a8, b8, lane, cs, cq);
+          float csum, cq;
+          transpose_reduce8(a8, b8, lane, csum, cq);
           if ((lane & 3) == 0) {
             const int col = cc * 8 + transpose_reduce8_col(lane);
-            ws[2 * col] += cs;
+            ws[2 * col] += csum;
             ws[2 * col + 1] += cq;
           }
         }
       }
-      tc::fence_before_sync();
-      tc::mbar_arrive(&acc_empty[buf]);
     }
-    if (p.sp.buf && group >= 0) stats_flush(p.sp, ws, 2 * NT, group, q, lane, 0, NT);
-  }
-  __syncthreads();
-  if (warp == 4) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, p.tmem_cols);
+    if (p.sp.buf && group >= 0) {
+      tc::wg_bar(8 + g);
+      if (half == 0) stats_flush(p.sp, ws, 2 * NT, group, q, lane, 0, NT);
+    }
   }
 }
 
+// N tile: the widest compiled width that divides the padded Cout (NT / 2 accumulator registers per consumer thread)
 static int cg_nt(int cout_pad) {
-  for (int nt = 256; nt >= 16; nt -= 16)
+  constexpr int kWidths[6] = {128, 96, 64, 48, 32, 16};
+  for (int nt : kWidths)
     if (cout_pad % nt == 0) return nt;
   return 16;
+}
+
+template <int NT>
+static int cg_launch(const CgParams& p, long long total_tiles, cudaStream_t st) {
+  const int smem = kCgStages * (kCgAStage + kCgUnits * NT * 32) + 128 + 4 * 2 * NT * 4 + 2 * 2 * tc::kStageFloats * 4 + 128;
+  // per-device attribute: set on every call (cheap), so a second GPU in the same process works
+  B200_CUDA(cudaFuncSetAttribute(conv_gather_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  dim3 grid((unsigned)std::min<long long>(total_tiles, num_sms()));
+  conv_gather_tc_kernel<NT><<<grid, 384, smem, st>>>(p);
+  B200_LAUNCH_CHECK("conv_gather_tc_kernel");
+  return B200_OK;
 }
 
 static int cg_setup(const b200_conv_gather_desc& d, CgParams& p) {
@@ -339,7 +322,6 @@ static int cg_setup(const b200_conv_gather_desc& d, CgParams& p) {
   p.d = d;
   p.cout_pad = (d.Cout + 15) / 16 * 16;
   p.NT = cg_nt(p.cout_pad);
-  p.tmem_cols = 2 * p.NT <= 32 ? 32 : 2 * p.NT <= 64 ? 64 : 2 * p.NT <= 128 ? 128 : 2 * p.NT <= 256 ? 256 : 512;
   cg_build_taps(d, p);
   if (d.transposed) {
     p.Dc = ceil_div(d.Do, d.stride); p.Hc = ceil_div(d.Ho, d.stride); p.Wc = ceil_div(d.Wo, d.stride);
@@ -399,9 +381,6 @@ extern "C" int b200_conv_gather_tc(const b200_conv_gather_desc* desc, const void
                  "conv_gather_tc: output shape does not match transposed-conv arithmetic");
   }
   p.x = (const __half*)x; p.w = (const __half*)packed_w; p.bias = bias; p.y = y;
-  const int smem = kCgStages * (kCgAStage + kCgUnits * p.NT * 32) + 128 + 4 * 2 * p.NT * 4 + 128;
-  // per-device attribute: set on every call (cheap), so a second GPU in the same process works
-  B200_CUDA(cudaFuncSetAttribute(conv_gather_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   const long long coarse = (long long)p.Dc * p.Hc * p.Wc;
   const long long tpg = (long long)p.ncls * ((coarse + 127) / 128), groups = (long long)d.N * (p.cout_pad / p.NT);
   const long long total_tiles = tpg * groups;
@@ -409,9 +388,15 @@ extern "C" int b200_conv_gather_tc(const b200_conv_gather_desc* desc, const void
   p.sp.R = stats_rows(tpg, total_tiles);
   p.sp.tiles_per_group = tpg;
   p.sp.rows_per_cta = 4;
-  dim3 grid((unsigned)std::min<long long>(total_tiles, num_sms()));
-  conv_gather_tc_kernel<<<grid, 288, smem, (cudaStream_t)stream>>>(p);
-  B200_LAUNCH_CHECK("conv_gather_tc_kernel");
+  switch (p.NT) {
+    case 128: rc = cg_launch<128>(p, total_tiles, (cudaStream_t)stream); break;
+    case 96: rc = cg_launch<96>(p, total_tiles, (cudaStream_t)stream); break;
+    case 64: rc = cg_launch<64>(p, total_tiles, (cudaStream_t)stream); break;
+    case 48: rc = cg_launch<48>(p, total_tiles, (cudaStream_t)stream); break;
+    case 32: rc = cg_launch<32>(p, total_tiles, (cudaStream_t)stream); break;
+    default: rc = cg_launch<16>(p, total_tiles, (cudaStream_t)stream); break;
+  }
+  if (rc) return rc;
   if (stats) return launch_stats_finish((const float*)workspace, groups, p.sp.R * 4, p.NT, p.cout_pad / p.NT, d.Cout, stats, (cudaStream_t)stream);
   return B200_OK;
 }

@@ -1,32 +1,29 @@
-// 3x3x3 stride-1 implicit-GEMM convolution on tcgen05 tensor cores (SURVEY.md §8 rows a8, a14).
+// 3x3x3 stride-1 implicit-GEMM convolution on Hopper wgmma tensor cores (SURVEY.md §8 rows a8, a14).
 //
 // Replaces the nn.Conv3d inside UnetResBlock / Convolution (monai/networks/blocks/dynunet_block.py:25-111,
 // monai/networks/blocks/convolutions.py:131-152) for kernel 3, stride 1, zero padding 1.
 //
 // Data layout in HBM ("NC8"): activations are fp16 [N][C/8][D][H][W][8]: eight channels of one voxel are 16
 // contiguous bytes and voxels run along W.  A shared-memory image of a (D,H,W) box of one 8-channel chunk is
-// then exactly a column of UMMA "core matrices" (8 rows x 16 B) for the K-major / no-swizzle operand layout:
+// then exactly a column of wgmma "core matrices" (8 rows x 16 B) for the K-major / no-swizzle operand layout:
 //   rows = 8 consecutive voxels along W, K = 8 channels.
 //
 // GEMM view: M = 128 output voxels (one 16(H) x 8(W) patch of one D-plane), N = NT output channels, K = 27*Cin.
 // Per K-slice of 16 input channels the CTA stages ONE halo tile (BD+2) x 18 x 10 voxels with a single 5-D TMA
-// box load (out-of-bounds => zero fill == the convolution's zero padding) and issues the taps as UMMA instructions
+// box load (out-of-bounds => zero fill == the convolution's zero padding) and issues the taps as wgmma instructions
 // whose A descriptors merely start at a shifted voxel of that tile (start += ((plane*18+kh)*10+kw)*16 B,
 // SBO = 10*16 B between the 16 row groups, LBO = chunk stride).  Weights are pre-packed into the exact B-operand
-// image and arrive by 1-D bulk copies (one (kh, kw) tap image per ring stage).  fp32 accumulators live in TMEM (one or
-// two sets of BD planes x NT columns); the epilogue reads them back with tcgen05.ld, adds bias, reduces InstanceNorm
+// image and arrive by 1-D bulk copies (one (kh, kw) tap image per ring stage).  fp32 accumulators (BD planes x NT
+// columns) live in the registers of two consumer warpgroups, 64 rows each; their epilogue adds bias, reduces InstanceNorm
 // partial sums and stores fp16 NC8.  The kernel is persistent: one CTA per SM walks the tile list (see the kernel).
 //
-// Depth-fused N: with the operands in shared memory an MMA of N = 48 is bound by the 4 KB A read, not by the tensor
-// pipe (24 cycles of math against ~44 cycles of operand traffic).  The loop therefore walks the INPUT planes of the
-// halo tile: input plane ip feeds output planes ip-kd (kd = 0..2), whose accumulators are adjacent TMEM column
-// blocks, so one MMA with the weights of kd = 2,1,0 stacked along N (N up to 3*NT <= 256) replaces three -- the A
-// tile is read once per (plane, kh, kw) instead of once per tap.
+// Depth blocking: a tile holds BD output planes, so each staged halo tile (BD + 2 input planes) serves the 3 x BD
+// (plane, kd) pairs of a (kh, kw) tap -- the halo is read from HBM once per BD planes instead of once per plane.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer, warps 2-5 = epilogue; with the
-// fused input normalisation (NORM, see the kernel) eight more warps rewrite each staged halo tile in place.
+// Warp roles (384 threads): warp 0 = TMA producer, warps 4-11 = two consumer warpgroups (MMA + epilogue); with the
+// fused input normalisation (NORM, see the kernel) warps 1-3 rewrite each staged halo tile in place.
 #include "common.cuh"
-#include "tc05.cuh"
+#include "tc90.cuh"
 #include "conv_epi.cuh"
 #include "../../include/monai_b200.h"
 #include <mutex>
@@ -124,23 +121,19 @@ struct ConvTcCfg {
   static constexpr int kABytes = 2 * kChunkBytes;                // 16 input channels
   static constexpr int kBTapBytes = 3 * NT * 32;                 // one (kh, kw): the three kd taps stacked along N, 3*NT x 16 fp16
   // weight ring: one (kh, kw) tap image per stage, ~44 KB in flight so a bulk copy has > 1 us to land before its
-  // MMAs are due (the ring, not the tensor pipe, was the limiter with three 9-tap slabs)
+  // MMAs are due
   static constexpr int kSB = (45056 / kBTapBytes) > 9 ? 9 : ((45056 / kBTapBytes) < 3 ? 3 : (45056 / kBTapBytes));
   static constexpr int kSA = 4;                                  // halo tiles in flight (one CTA per SM owns the whole shared memory)
-  static constexpr int kKdGroup = (3 * NT <= 256) ? 3 : ((2 * NT <= 256) ? 2 : 1);   // kd taps fused into one MMA (UMMA N <= 256)
-  // RES: the 1x1x1 residual convolution of UnetResBlock is folded in (see the kernel): a second block of BD planes x NT columns per set
-  static constexpr int kAccSet = (RES ? 2 : 1) * BD * NT;        // TMEM columns of one accumulator set
-  static constexpr int kAccBufs = (2 * kAccSet <= 512) ? 2 : 1;  // accumulator sets: 2 lets the epilogue of tile i overlap the MMAs of tile i+1
-  static constexpr int kAccCols = kAccBufs * kAccSet;
-  static constexpr int kTmemCols = (kAccCols <= 32) ? 32 : (kAccCols <= 64) ? 64 : (kAccCols <= 128) ? 128 : (kAccCols <= 256) ? 256 : 512;
+  // RES: the 1x1x1 residual convolution of UnetResBlock is folded in (see the kernel): a second block of BD planes x NT columns
+  static constexpr int kAccSet = (RES ? 2 : 1) * BD * NT;        // accumulator columns of a tile (kAccSet / 2 registers per thread)
   static constexpr int kRBytes = NT * 32;                        // RES: the 1x1x1 weights of one K slice (NT x 16 fp16), 2 stages
   static constexpr int kSR = 2;
-  static constexpr int kResEG = BD >= 2 ? 2 : 1;                 // RES: epilogue warp groups (they split the planes of a tile)
-  static constexpr int kThreads = RES ? 64 + 128 * kResEG : 192; // (+ 256 transform threads with NORM, see the kernel)
+  static constexpr int kThreads = 384;                           // producer warpgroup + two consumer warpgroups
+  static constexpr int kStatRows = (RES ? 8 : 4);                // one row of running sums per 32-row quarter and output
   static constexpr int kSmemBytes = kSA * kABytes + kSB * kBTapBytes + (RES ? kSR * kRBytes : 0) + 384 /*barriers*/ +
-                                    (RES ? 8 * kResEG : 4) * 2 * NT * 4 /*warp-private stats rows*/ + 128 /*align slack*/;
-  static_assert(kAccSet <= 512, "accumulators exceed TMEM");
-  static_assert(NT % 16 == 0 && NT >= 16 && NT <= 256, "invalid UMMA N");
+                                    kStatRows * 2 * NT * 4 + 2 * 2 * tc::kStageFloats * 4 /*slice buffers*/ + 128 /*align slack*/;
+  static_assert(kAccSet <= 256, "accumulators exceed the register budget of a consumer thread");
+  static_assert(NT % 16 == 0 && NT >= 16 && NT <= 256, "invalid wgmma N");
   static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
 };
 
@@ -153,27 +146,27 @@ struct ConvTcParams {
   const __half* res_w;     // RES: packed 1x1x1 weights (gemm_tc image: [nt][k16][khalf][NT/8][8][8])
 };
 
-// Persistent, warp-specialised (192 threads, one CTA per SM): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer,
-// warps 2-5 = epilogue.  Each CTA walks tiles blockIdx.x, blockIdx.x + gridDim.x, ...; the shared-memory rings run
-// across tile boundaries and (when 2*BD*NT <= 512 columns) two TMEM accumulator sets alternate.
+// Persistent, warp-specialised (384 threads, one CTA per SM): warp 0 = TMA producer, warps 4-7 and 8-11 = two consumer
+// warpgroups that run the wgmma chain of rows 0-63 / 64-127 of every tile with the fp32 accumulators in registers and then
+// its epilogue.  Each CTA walks tiles blockIdx.x, blockIdx.x + gridDim.x, ...; the shared-memory rings run across tile
+// boundaries, so the loads of tile i+1 are in flight during the epilogue of tile i.
 //
-// NORM (448 threads): the input is the RAW output of the previous convolution and InstanceNorm + activation
-// (monai/networks/blocks/dynunet_block.py:97-103: conv1 -> norm1 -> lrelu -> conv2) is applied on the operand load: warps 6-13
+// NORM: the input is the RAW output of the previous convolution and InstanceNorm + activation
+// (monai/networks/blocks/dynunet_block.py:97-103: conv1 -> norm1 -> lrelu -> conv2) is applied on the operand load: warps 1-3
 // rewrite every staged halo tile in place -- y = act(x * rstd - mean * rstd), the exact expression and rounding of
 // norm_act_nc8_kernel, so the MMAs consume bit-identical fp16 operands -- between the TMA completion (full_a) and the MMAs
 // (ready_a).  Voxels outside the volume keep the TMA's zero fill: the convolution pads the NORMALISED tensor with zeros.
-// This removes one read and one write of the activation tensor per residual block (norm_act_nc8: 102 ms per C3 step).
+// This removes one read and one write of the activation tensor per residual block.
 //
 // RES: the 1x1x1 convolution of the residual branch (UnetResBlock.conv3, dynunet_block.py:75-87, 104-108) reads the SAME input as
 // conv1, so it is folded into this kernel: per K slice one extra MMA per output plane multiplies the centre view of the staged
 // halo tile (kh = kw = 1 of input plane o + 1) with the 1x1x1 weights into a second accumulator block, and the epilogue stores
-// both tensors with their statistics (conv_epilogue_res).  This deletes a launch that re-read the 2 x C input tensor
-// (decoder1 of SwinUNETR: 6.4 GB per 25 windows, 2.3 ms at 2.8 TB/s); the price is a single accumulator set at NT = 48, BD = 4.
+// both tensors with their statistics.  This deletes a launch that re-reads the 2 x C input tensor.
 template <int NT, int BD, bool NORM, bool RES>
-__global__ void __launch_bounds__(NORM ? 448 : ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3_tc_kernel(const __grid_constant__ CUtensorMap tmap, ConvTcParams p) {
+__global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3_tc_kernel(const __grid_constant__ CUtensorMap tmap, ConvTcParams p) {
   using Cfg = ConvTcCfg<NT, BD, RES>;
   static_assert(!(NORM && RES), "the residual fold is used by conv1, the operand normalisation by conv2");
-  constexpr int kSA = Cfg::kSA, kSB = Cfg::kSB, kNB = Cfg::kAccBufs;
+  constexpr int kSA = Cfg::kSA, kSB = Cfg::kSB;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = tc::align_smem128(smem_raw);   // keeps the shared address space (LDS/STS, not generic LD/ST)
   uint8_t* smem_a = smem;
@@ -184,35 +177,25 @@ __global__ void __launch_bounds__(NORM ? 448 : ConvTcCfg<NT, BD, RES>::kThreads,
   uint64_t* empty_a = bars + kSA;       // [kSA]
   uint64_t* full_b = bars + 2 * kSA;    // [kSB]
   uint64_t* empty_b = full_b + kSB;     // [kSB]
-  uint64_t* acc_full = empty_b + kSB;   // [2]
-  uint64_t* acc_empty = acc_full + 2;   // [2]
-  uint64_t* ready_a = acc_empty + 2;    // [kSA] NORM: 8 arrivals (one per transform warp)
+  uint64_t* ready_a = empty_b + kSB;    // [kSA] NORM: 3 arrivals (one per transform warp)
   uint64_t* full_r = ready_a + kSA;     // [2] RES
   uint64_t* empty_r = full_r + 2;       // [2] RES
-  uint64_t* res_empty = empty_r + 2;    // [2] RES: the residual accumulator block has been drained
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_empty + 2);
-  static_assert(3 * kSA + 2 * kSB + 4 + 6 + 1 <= 48, "barrier block");
-  float* s_stats = reinterpret_cast<float*>(bars + 48);  // [4][2*NT]
+  static_assert(3 * kSA + 2 * kSB + 4 <= 48, "barrier block");
+  float* s_stats = reinterpret_cast<float*>(bars + 48);  // [kStatRows][2*NT]
+  float* s_stage = s_stats + Cfg::kStatRows * 2 * NT;    // [2 warpgroups][2][kStageFloats]
 
   const b200_conv_tc_desc& d = p.d;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int num_kc = d.Cin / 16;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kSA; ++i) { tc::mbar_init(&full_a[i], 1); tc::mbar_init(&empty_a[i], 1); tc::mbar_init(&ready_a[i], 8); }
-    for (int i = 0; i < kSB; ++i) { tc::mbar_init(&full_b[i], 1); tc::mbar_init(&empty_b[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&acc_full[i], 1); tc::mbar_init(&acc_empty[i], RES ? 4 * Cfg::kResEG : 4);
-      tc::mbar_init(&full_r[i], 1); tc::mbar_init(&empty_r[i], 1); tc::mbar_init(&res_empty[i], 4 * Cfg::kResEG);
-    }
+    for (int i = 0; i < kSA; ++i) { tc::mbar_init(&full_a[i], 1); tc::mbar_init(&empty_a[i], 2); tc::mbar_init(&ready_a[i], 3); }
+    for (int i = 0; i < kSB; ++i) { tc::mbar_init(&full_b[i], 1); tc::mbar_init(&empty_b[i], 2); }
+    for (int i = 0; i < 2; ++i) { tc::mbar_init(&full_r[i], 1); tc::mbar_init(&empty_r[i], 2); }
     tc::fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < (RES ? 8 * Cfg::kResEG : 4) * 2 * NT; i += blockDim.x) s_stats[i] = 0.f;
-  if (warp == 1) tc::tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc::fence_before_sync();
+  for (int i = threadIdx.x; i < Cfg::kStatRows * 2 * NT; i += blockDim.x) s_stats[i] = 0.f;
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ===================== TMA producer =====================
@@ -245,174 +228,140 @@ __global__ void __launch_bounds__(NORM ? 448 : ConvTcCfg<NT, BD, RES>::kThreads,
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // The whole warp runs the loop control (converged, so addresses and descriptors stay on the uniform datapath); one
-    // elected lane issues the tcgen05 instructions.
-    {
-      constexpr int G = Cfg::kKdGroup;
-      const bool leader = tc::elect_one();
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-      int sa = 0, sb = 0, sr = 0; uint32_t pa = 0, pb = 0, pr = 0;
-      uint32_t a_base = 0, tacc = 0;
-      // RES: D_res[plane o] (+)= centre view of input plane o + 1 x W3 slice; FIRST (first K slice) initialises the accumulators
-      auto residual = [&](auto first_c) {
-        constexpr bool FIRST = decltype(first_c)::value;
-        tc::mbar_wait(&full_r[sr], pr);
-        tc::fence_after_sync();
-        const uint64_t bdesc = tc::make_desc_kmajor_noswz(tc::smem_u32(smem_r + sr * Cfg::kRBytes), NT * 16, 128);
-#pragma unroll
-        for (int o = 0; o < BD; ++o) {
-          const uint64_t adesc = tc::make_desc_kmajor_noswz(a_base + (((o + 1) * kHH + 1) * kHW + 1) * 16, Cfg::kChunkBytes, kHW * 16);
-          if (leader) tc::mma_f16_ss(tacc + BD * NT + o * NT, adesc, bdesc, tc::make_idesc_f16(128, NT), FIRST ? 0u : 1u);
-        }
-        if (leader) tc::mma_commit(&empty_r[sr]);
-        __syncwarp();
-        if (++sr == Cfg::kSR) { sr = 0; pr ^= 1; }
-      };
-      // One (kh, kw) tap of one K-slice: every input plane ip of the halo tile feeds output planes ip - kd.  FIRST is the
-      // very first tap of the tile: it initialises the accumulators, so it issues one MMA per (plane, kd) with a
-      // static accumulate flag; every other tap fuses the kd range of a plane into one MMA.  (Kept as two separately
-      // instantiated bodies: a run-time "first" flag made ptxas merge the two forms into predicated code.)
-      auto tap = [&](auto first_c, int kh, int kw) {
-        constexpr bool FIRST = decltype(first_c)::value;
+  } else if (warp >= 4) {
+    // ===================== consumers: wgmma + epilogue =====================
+    const int g = (warp >> 2) - 1, wid = warp & 3;
+    const bool leader = wid == 0 && lane == 0;
+    const int q = 2 * g + (wid & 1);
+    float* stage = s_stage + g * 2 * tc::kStageFloats;
+    float* ws_m = s_stats + q * (2 * NT);
+    float* ws_r = s_stats + (4 + q) * (2 * NT);
+    int sa = 0, sb = 0, sr = 0; uint32_t pa = 0, pb = 0, pr = 0;
+    int prev_sb = -1;
+    int sl = 0;
+    long long group_m = -1, group_r = -1;
+    for (long long t = blockIdx.x; t < p.e.total_tiles; t += gridDim.x) {
+      const ConvTile c = conv_tile<BD>(p.e, t);
+      float acc[Cfg::kAccSet / 2];
+      uint32_t a_base = 0;
+      // One (kh, kw) tap of one K-slice: every input plane ip of the halo tile feeds output planes ip - kd.  One NT-wide MMA per
+      // (ip, kd): in-flight wgmma instructions are ordered only between instructions of the same shape on the same
+      // accumulator registers, so the kd taps of a plane are not fused into one wider MMA (that would write overlapping
+      // register ranges at different offsets).  A plane accumulates kd = 0, 1, 2 in ip order; the accumulators start at zero.
+      // The B stage of the previous tap is released as soon as its MMAs have completed (one wgmma group stays in flight).
+      auto tap = [&](int kh, int kw) {
         tc::mbar_wait(&full_b[sb], pb);
-        tc::fence_after_sync();
         const uint32_t b_tap = tc::smem_u32(smem_b + sb * Cfg::kBTapBytes);
-#pragma unroll
-        for (int ip = 0; ip < BD + 2; ++ip) {
-          const int kd_hi = ip < 2 ? ip : 2, kd_lo = ip - (BD - 1) > 0 ? ip - (BD - 1) : 0;
+        tc::wg_fence();
+        tc::static_for<0, BD + 2>([&](auto ipc) {
+          constexpr int ip = decltype(ipc)::value;
+          constexpr int kd_hi = ip < 2 ? ip : 2, kd_lo = ip - (BD - 1) > 0 ? ip - (BD - 1) : 0;
           const uint32_t a_addr = a_base + ((ip * kHH + kh) * kHW + kw) * 16;
           const uint64_t adesc = tc::make_desc_kmajor_noswz(a_addr, Cfg::kChunkBytes, kHW * 16);
-          if constexpr (FIRST) {
-#pragma unroll
-            for (int kd = 2; kd >= 0; --kd) {
-              if (kd > kd_hi || kd < kd_lo) continue;
+          tc::static_for<0, 3>([&](auto kdc) {
+            constexpr int kd = 2 - decltype(kdc)::value;
+            if constexpr (kd <= kd_hi && kd >= kd_lo) {
               const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_tap + (2 - kd) * NT * 16, 3 * NT * 16, 128);
-              // plane ip - kd was initialised when it was the kd = 0 plane of an earlier ip
-              if (leader) tc::mma_f16_ss(tacc + (ip - kd) * NT, adesc, bdesc, tc::make_idesc_f16(128, NT), kd != 0 ? 1u : 0u);
+              tc::wg_mma_ss<NT>(acc + (ip - kd) * NT / 2, adesc, bdesc, 1u, 128);
             }
-          } else {
-#pragma unroll
-            for (int top = 2; top >= 0; top -= G) {   // kd groups [top-G+1, top] clipped to [kd_lo, kd_hi]
-              const int hi = top < kd_hi ? top : kd_hi, lo = (top - G + 1) > kd_lo ? (top - G + 1) : kd_lo;
-              if (hi < lo) continue;
-              const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_tap + (2 - hi) * NT * 16, 3 * NT * 16, 128);
-              if (leader) tc::mma_f16_ss(tacc + (ip - hi) * NT, adesc, bdesc, tc::make_idesc_f16(128, (hi - lo + 1) * NT), 1u);
-            }
-          }
-        }
-        if (leader) tc::mma_commit(&empty_b[sb]);
-        __syncwarp();
+          });
+        });
+        tc::wg_commit();
+        tc::wg_wait<1>();
+        if (prev_sb >= 0 && leader) tc::mbar_arrive(&empty_b[prev_sb]);
+        prev_sb = sb;
         if (++sb == kSB) { sb = 0; pb ^= 1; }
       };
-      int it = 0;
-      for (long long t = blockIdx.x; t < p.e.total_tiles; t += gridDim.x, ++it) {
-        const int buf = it % kNB;
-        const uint32_t aph = (uint32_t)((it / kNB) & 1);
-        tc::mbar_wait(&acc_empty[buf], aph ^ 1);   // the epilogue has drained this accumulator set
-        tc::fence_after_sync();
-        tacc = tmem_u + buf * Cfg::kAccSet;
-        for (int kc = 0; kc < num_kc; ++kc) {
-          tc::mbar_wait(NORM ? &ready_a[sa] : &full_a[sa], pa);
-          tc::fence_after_sync();
-          a_base = tc::smem_u32(smem_a + sa * Cfg::kABytes);
-          if (kc == 0) tap(std::true_type{}, 0, 0);
-          else tap(std::false_type{}, 0, 0);
+      // RES: D_res[plane o] += centre view of input plane o + 1 x W3 slice
+      auto residual = [&]() {
+        tc::mbar_wait(&full_r[sr], pr);
+        const uint64_t bdesc = tc::make_desc_kmajor_noswz(tc::smem_u32(smem_r + sr * Cfg::kRBytes), NT * 16, 128);
+        tc::wg_fence();
+        tc::static_for<0, BD>([&](auto oc) {
+          constexpr int o = decltype(oc)::value;
+          const uint64_t adesc = tc::make_desc_kmajor_noswz(a_base + (((o + 1) * kHH + 1) * kHW + 1) * 16, Cfg::kChunkBytes, kHW * 16);
+          tc::wg_mma_ss<NT>(acc + (BD * NT + o * NT) / 2, adesc, bdesc, 1u, 128);
+        });
+        tc::wg_commit();
+      };
 #pragma unroll
-          for (int t9 = 1; t9 < 9; ++t9) tap(std::false_type{}, t9 / 3, t9 % 3);
-          if constexpr (RES) {
-            if (kc == 0) {
-              tc::mbar_wait(&res_empty[buf], aph ^ 1);   // the epilogue has drained the residual block of this set
-              tc::fence_after_sync();
-              residual(std::true_type{});
-            } else {
-              residual(std::false_type{});
-            }
-          }
-          if (leader) tc::mma_commit(&empty_a[sa]);
-          __syncwarp();
-          if (++sa == kSA) { sa = 0; pa ^= 1; }
+      for (int i = 0; i < Cfg::kAccSet / 2; ++i) acc[i] = 0.f;
+      for (int kc = 0; kc < num_kc; ++kc) {
+        tc::mbar_wait(NORM ? &ready_a[sa] : &full_a[sa], pa);
+        a_base = tc::smem_u32(smem_a + sa * Cfg::kABytes) + g * 8 * kHW * 16;   // rows 64.. = patch rows h0 + 8 ..
+#pragma unroll 1
+        for (int t9 = 0; t9 < 9; ++t9) tap(t9 / 3, t9 % 3);
+        if constexpr (RES) residual();
+        tc::wg_wait<0>();
+        tc::wg_fence_acc<Cfg::kAccSet / 2>(acc);
+        if (leader) {
+          tc::mbar_arrive(&empty_b[prev_sb]);
+          tc::mbar_arrive(&empty_a[sa]);
+          if constexpr (RES) tc::mbar_arrive(&empty_r[sr]);
         }
-        if (leader) tc::mma_commit(&acc_full[buf]);
-        __syncwarp();
+        prev_sb = -1;
+        if constexpr (RES) { if (++sr == Cfg::kSR) { sr = 0; pr ^= 1; } }
+        if (++sa == kSA) { sa = 0; pa ^= 1; }
+      }
+      conv_stats_turn(p.e, ws_m, NT, t, group_m, g, wid, lane);
+      conv_epilogue<NT, BD>(p.e, c, acc, stage, ws_m, g, wid, lane, sl);
+      if constexpr (RES) {
+        conv_stats_turn(p.r, ws_r, NT, t, group_r, g, wid, lane);
+        conv_epilogue<NT, BD>(p.r, c, acc + BD * NT / 2, stage, ws_r, g, wid, lane, sl);
       }
     }
-    __syncwarp();
-  } else if (warp < (RES ? 2 + 4 * Cfg::kResEG : 6)) {
-    // ===================== epilogue (warps 2..5; RES: warps 2..9 in two groups) =====================
-    if constexpr (RES) conv_epilogue_res<NT, BD, kNB, Cfg::kResEG>(p.e, p.r, tmem_base, acc_full, acc_empty, res_empty, s_stats, warp, lane, (warp - 2) >> 2);
-    else conv_epilogue<NT, BD, kNB>(p.e, tmem_base, acc_full, acc_empty, s_stats, warp, lane);
+    conv_stats_final(p.e, ws_m, NT, group_m, g, wid, lane);
+    if constexpr (RES) conv_stats_final(p.r, ws_r, NT, group_r, g, wid, lane);
   } else if constexpr (NORM) {
-    // ===================== operand transform (warps 6..13): InstanceNorm + activation in place =====================
-    // 256 threads: 128 per 8-channel chunk; four vectors are loaded before the first is converted (one warp per scheduler with
-    // a load -> convert -> store chain per vector left the tensor pipe waiting: 37 % active against 65 % without the fusion)
-    const int tt = threadIdx.x - 192;                      // 0..255
-    const int chunk = tt >> 7, t128 = tt & 127;
+    // ===================== operand transform (warps 1-3): InstanceNorm + activation in place =====================
+    const int tt = threadIdx.x - 32;                       // 0..95
     constexpr int kVox = Cfg::kPlanes * kHH * kHW;         // 16-byte voxel vectors per chunk image
-    constexpr int kIter = (kVox + 127) / 128;
     const float invS = 1.f / ((float)d.D * (float)d.H * (float)d.W);
     const float slope = d.in_act == 1 ? d.in_slope : (d.in_act == 3 ? 0.f : 1.f), eps = d.in_eps;
     int sa = 0; uint32_t pa = 0;
     for (long long t = blockIdx.x; t < p.e.total_tiles; t += gridDim.x) {
       const ConvTile c = conv_tile<BD>(p.e, t);
-      // which of this thread's vectors lie inside the volume (same for every K slice of the tile)
-      uint32_t inside = 0;
-#pragma unroll
-      for (int k = 0; k < kIter; ++k) {
-        const int v = t128 + 128 * k;
-        const int pz = v / (kHH * kHW), rem = v - pz * (kHH * kHW), py = rem / kHW, px = rem - py * kHW;
-        const int gz = c.d0 - 1 + pz, gy = c.h0 - 1 + py, gx = c.w0 - 1 + px;
-        if (v < kVox && (unsigned)gz < (unsigned)d.D && (unsigned)gy < (unsigned)d.H && (unsigned)gx < (unsigned)d.W) inside |= 1u << k;
-      }
       for (int kc = 0; kc < num_kc; ++kc) {
-        float sc[8], sh[8];
+        float sc[16], sh[16];
         {
-          const float* st = p.in_stats + 2 * ((long long)c.n * d.Cin + kc * 16 + chunk * 8);
+          const float* st = p.in_stats + 2 * ((long long)c.n * d.Cin + kc * 16);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
+          for (int j = 0; j < 16; ++j) {
             const float sm = __ldg(st + 2 * j), q = __ldg(st + 2 * j + 1);
             const float mean = sm * invS, var = fmaxf(q * invS - mean * mean, 0.f), rstd = 1.f / sqrtf(var + eps);
             sc[j] = rstd; sh[j] = -mean * rstd;
           }
         }
         tc::mbar_wait(&full_a[sa], pa);
-        uint8_t* img = smem_a + sa * Cfg::kABytes + chunk * Cfg::kChunkBytes + t128 * 16;
-        auto xform = [&](uint4& raw) {
-          __half2* h2 = reinterpret_cast<__half2*>(&raw);
+        uint8_t* img = smem_a + sa * Cfg::kABytes;
+#pragma unroll 2
+        for (int v = tt; v < 2 * kVox; v += 96) {
+          const int chunk = v >= kVox ? 1 : 0, vi = v - chunk * kVox;
+          const int pz = vi / (kHH * kHW), rem = vi - pz * (kHH * kHW), py = rem / kHW, px = rem - py * kHW;
+          const int gz = c.d0 - 1 + pz, gy = c.h0 - 1 + py, gx = c.w0 - 1 + px;
+          if ((unsigned)gz < (unsigned)d.D && (unsigned)gy < (unsigned)d.H && (unsigned)gx < (unsigned)d.W) {
+            uint4* ptr = reinterpret_cast<uint4*>(img + chunk * Cfg::kChunkBytes + vi * 16);
+            uint4 raw = *ptr;
+            __half2* h2 = reinterpret_cast<__half2*>(&raw);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float2 f = __half22float2(h2[j]);
-            const float a = fmaf(f.x, sc[2 * j], sh[2 * j]), b = fmaf(f.y, sc[2 * j + 1], sh[2 * j + 1]);
-            // one branch-free form for none / leaky-relu / relu: max(a, a * s) with s = 1 / slope / 0 (0 <= slope <= 1) returns
-            // exactly what `a >= 0 ? a : a * slope` returns
-            h2[j] = __floats2half2_rn(fmaxf(a, a * slope), fmaxf(b, b * slope));
-          }
-        };
-#pragma unroll
-        for (int k0 = 0; k0 < kIter; k0 += 4) {
-          uint4 raw[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (k0 + u < kIter && (inside >> (k0 + u) & 1u)) raw[u] = *reinterpret_cast<const uint4*>(img + (k0 + u) * 2048);
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (k0 + u < kIter && (inside >> (k0 + u) & 1u)) {
-              xform(raw[u]);
-              *reinterpret_cast<uint4*>(img + (k0 + u) * 2048) = raw[u];
+            for (int j = 0; j < 4; ++j) {
+              const float2 f = __half22float2(h2[j]);
+              const float s0 = chunk ? sc[8 + 2 * j] : sc[2 * j], s1 = chunk ? sc[9 + 2 * j] : sc[2 * j + 1];
+              const float o0 = chunk ? sh[8 + 2 * j] : sh[2 * j], o1 = chunk ? sh[9 + 2 * j] : sh[2 * j + 1];
+              const float a = fmaf(f.x, s0, o0), b = fmaf(f.y, s1, o1);
+              // one branch-free form for none / leaky-relu / relu: max(a, a * s) with s = 1 / slope / 0 (0 <= slope <= 1) returns
+              // exactly what `a >= 0 ? a : a * slope` returns
+              h2[j] = __floats2half2_rn(fmaxf(a, a * slope), fmaxf(b, b * slope));
             }
+            *ptr = raw;
+          }
         }
-        tc::fence_proxy_async();       // generic-proxy stores -> visible to tcgen05.mma
+        tc::fence_proxy_async();       // generic-proxy stores -> visible to the wgmma operand reads
         __syncwarp();                  // one arrival per warp
         if (lane == 0) tc::mbar_arrive(&ready_a[sa]);
         if (++sa == kSA) { sa = 0; pa ^= 1; }
       }
     }
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, Cfg::kTmemCols);
   }
 }
 
@@ -539,7 +488,7 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
   ConvTcGeom<NT, BD>::fill(d, p.e);
   const long long sp_tiles = (long long)p.e.tiles_w * p.e.tiles_h * p.e.tiles_d, groups = (long long)d.N * p.e.n_tiles;
   const int R = stats_rows(sp_tiles, p.e.total_tiles);
-  constexpr int kRows = RES ? 4 * Cfg::kResEG : 4;                 // partial rows a CTA writes per group
+  constexpr int kRows = 4;                                          // partial rows a CTA writes per group (one per quarter)
   const long long one = stats_partial_bytes(groups, R, NT, kRows);
   c.ws_bytes = RES ? 2 * one : one;     // RES: main partials, then the residual's
   if (c.query) return B200_OK;
@@ -567,7 +516,7 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
   auto kern = conv3x3x3_tc_kernel<NT, BD, NORM, RES>;
   // per-device attribute: set on every call (cheap), so a second GPU in the same process works
   B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  kern<<<grid, NORM ? 448 : Cfg::kThreads, Cfg::kSmemBytes, c.st>>>(tmap, p);
+  kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, c.st>>>(tmap, p);
   B200_LAUNCH_CHECK("conv3x3x3_tc_kernel");
   if (c.stats) {
     const int rc = launch_stats_finish((const float*)c.ws, groups, R * kRows, NT, p.e.n_tiles, d.Cout, c.stats, c.st);
@@ -580,7 +529,7 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
 template <int NT, int BD>
 static int launch_variant(const b200_conv_tc_desc& d, ConvTcCall& c) {
   if (d.in_stats) return launch_conv_tc<NT, BD, true>(d, c);
-  if constexpr (NT <= 128) {
+  if constexpr (NT <= 128 && 2 * BD * NT <= 256) {
     if (d.res_w) return launch_conv_tc<NT, BD, false, true>(d, c);
   }
   return launch_conv_tc<NT, BD, false>(d, c);
@@ -588,15 +537,14 @@ static int launch_variant(const b200_conv_tc_desc& d, ConvTcCall& c) {
 
 template <int NT>
 static int dispatch_bd(const b200_conv_tc_desc& d, ConvTcCall& c) {
-  // deeper CTA tiles amortise the halo and fuse more kd taps per MMA; two accumulator sets (2*BD*NT <= 512 TMEM columns)
-  // let the epilogue overlap the next tile, which is worth more than depth for the wide-N layers
-  // A/B switch: B200_RES_BD2=1 runs the folded-residual variant with two planes per tile (two accumulator sets fit again)
-  static const bool res_bd2 = std::getenv("B200_RES_BD2") != nullptr;
-  if constexpr (2 * NT * 4 <= 512) {
-    if ((d.D % 4 == 0 || d.D >= 16) && !(res_bd2 && d.res_w)) return launch_variant<NT, 4>(d, c);
+  // deeper CTA tiles amortise the halo and fuse more kd taps per MMA; the depth is bounded by the accumulators a consumer
+  // thread can hold (BD * NT, twice that with the folded residual, <= 256 columns = 128 registers)
+  const int res = d.res_w ? 2 : 1;
+  if constexpr (NT * 4 <= 256) {
+    if ((d.D % 4 == 0 || d.D >= 16) && 4 * NT * res <= 256) return launch_variant<NT, 4>(d, c);
   }
-  if constexpr (NT * 2 <= 512) {
-    if (d.D >= 2) return launch_variant<NT, 2>(d, c);
+  if constexpr (NT * 2 <= 256) {
+    if (d.D >= 2 && 2 * NT * res <= 256) return launch_variant<NT, 2>(d, c);
   }
   return launch_variant<NT, 1>(d, c);
 }

@@ -1,4 +1,4 @@
-// Y = epilogue( X * W^T ) on tcgen05 tensor cores for channel-blocked (NC8) activations (SURVEY.md §8 rows a8, a12, a13).
+// Y = epilogue( X * W^T ) on Hopper wgmma tensor cores for channel-blocked (NC8) activations (SURVEY.md §8 rows a8, a12, a13).
 //
 // One kernel serves every GEMM-shaped layer of SwinUNETR outside the 3x3x3 convolutions:
 //   * nn.Linear of WindowAttention.qkv / proj, MLPBlock.linear1 / linear2, PatchMerging.reduction
@@ -8,13 +8,13 @@
 //     scatter of each (tap, cout) group to the 2x-upsampled voxel.
 //
 // Operands: X is NC8 [Nb][K/8][S][8] fp16 (rows = S tokens/voxels); a 128-row A tile of one 8-channel chunk is 2 KB
-// contiguous in HBM and lands in shared memory as the UMMA K-major / no-swizzle core-matrix column
+// contiguous in HBM and lands in shared memory as the wgmma K-major / no-swizzle core-matrix column
 // (LBO = 128*16 B between K chunks, SBO = 128 B between 8-row groups).  W is pre-packed into the B image
-// [nt][k16][khalf][NT/8][8][8] and streamed with 1-D bulk copies.  fp32 accumulators live in TMEM.
-// Epilogue (16 warps, four per TMEM lane quarter, variant chosen at compile time): + bias, GELU(erf), + residual,
+// [nt][k16][khalf][NT/8][8][8] and streamed with 1-D bulk copies.  fp32 accumulators live in the registers of two
+// consumer warpgroups.  Epilogue (variant chosen at compile time): + bias, GELU(erf), + residual,
 // InstanceNorm partial sums, and a row map (identity / index table / 2x upsample scatter) before the fp16 NC8 store.
 #include "common.cuh"
-#include "tc05.cuh"
+#include "tc90.cuh"
 #include "stats.cuh"
 #include "gelu.cuh"
 #include "../../include/monai_b200.h"
@@ -25,9 +25,20 @@ constexpr int kGemmStages = 4;
 constexpr int kGemmK16PerStage = 4;                 // 64 K elements per pipeline stage
 constexpr int kGemmAStage = kGemmK16PerStage * 2 * 128 * 16;  // 16 KB
 
+// Width of the packed weight tiles (b200_gemm_tc_pack_weight): the widest multiple of 16 up to 256 that divides N.  Other
+// kernels read these images too (the fused MLP, the folded residual of conv3x3x3_tc), so the packing does not depend on the
+// tile the GEMM kernel runs.
 __host__ __device__ inline int gemm_tc_nt(int N) {
   for (int nt = 256; nt >= 16; nt -= 16)
     if (N % nt == 0) return nt;
+  return 16;
+}
+// N tile of the GEMM kernel: the widest compiled width that divides the packing width P (the accumulator of a 64-row half
+// tile is NT / 2 registers per thread, so 128 is the widest that leaves room for the epilogue)
+__host__ __device__ inline int gemm_tile_n(int P) {
+  constexpr int kWidths[6] = {128, 96, 64, 48, 32, 16};
+  for (int nt : kWidths)
+    if (P % nt == 0) return nt;
   return 16;
 }
 
@@ -35,7 +46,7 @@ struct GemmTcParams {
   b200_gemm_tc_desc d;
   const __half* x; const __half* w; const float* bias; __half* y; const __half* res; const int32_t* row_map;
   StatsPartials sp;   // deterministic InstanceNorm partial sums (stats.cuh)
-  int NT, tmem_cols;
+  int P;              // width of the packed weight tiles (gemm_tc_nt(N)); the kernel's N tile divides it
 };
 
 __global__ void gemm_tc_pack_weight_kernel(const float* __restrict__ w, __half* __restrict__ out, int N, int K, int NT,
@@ -55,14 +66,13 @@ __global__ void gemm_tc_pack_weight_kernel(const float* __restrict__ w, __half* 
   }
 }
 
-// Persistent, warp-specialised: each CTA loops over (batch, row tile, N tile) work items.  Two TMEM accumulator
-// buffers let the epilogue of tile i overlap the MMAs of tile i+1; the shared-memory ring runs across tile boundaries.
-// The epilogue variant (row mapping, activation, residual, statistics) is a template parameter: the per-step
-// instruction stream is what bounds these HBM-shaped GEMMs, so nothing is decided at run time inside the column loop.
-constexpr int kGemmEpiWarps = 16;   // 4 per TMEM lane quarter; warps sharing a quarter split the 16-column steps
-constexpr int kGemmThreads = 64 + 32 * kGemmEpiWarps;
-
-using tc::tmem_ld_wait16;
+// Persistent, warp-specialised: each CTA loops over (batch, row tile, N tile) work items.  Warp 0 streams the operands
+// through a shared-memory ring that runs across tile boundaries; two consumer warpgroups (warps 4-7: rows 0-63, warps
+// 8-11: rows 64-127 of the 128-row tile) run the wgmma chain with the fp32 accumulators in registers and then the
+// epilogue of their rows.  The epilogue variant (row mapping, activation, residual, statistics) is a template parameter:
+// the per-step instruction stream is what bounds these HBM-shaped GEMMs, so nothing is decided at run time inside the
+// column loop.
+constexpr int kGemmThreads = 384;
 
 // tile -> (N tile, row tile, batch item).  Without statistics the N tiles of a row tile run back to back (the A tile is
 // re-read from L2); with statistics the row tiles of one (batch item, N tile) group are contiguous, which is what the
@@ -79,41 +89,39 @@ __device__ __forceinline__ void gemm_tile(long long tile, int n_tiles, int row_t
   n = (int)(tile / ((long long)n_tiles * row_tiles));
 }
 
-template <int MODE, int ACT, bool RES, bool STATS>
+template <int NT>
+__host__ __device__ constexpr int gemm_smem_bytes() {
+  return kGemmStages * (kGemmAStage + kGemmK16PerStage * NT * 32) + 128 /*barriers*/ + 4 * 2 * NT * 4 /*stats rows*/ +
+         2 * 2 * tc::kStageFloats * 4 /*slice buffers*/ + 128 /*align slack*/;
+}
+
+template <int NT, int MODE, int ACT, bool RES, bool STATS>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(GemmTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = tc::align_smem128(smem_raw);   // keeps the shared address space (LDS/STS, not generic LD/ST)
-  const int NT = p.NT;
-  const int b_stage = kGemmK16PerStage * NT * 32;
+  constexpr int b_stage = kGemmK16PerStage * NT * 32;
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kGemmStages * kGemmAStage;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + kGemmStages * b_stage);
   uint64_t* full = bars;
   uint64_t* empty = bars + kGemmStages;
-  uint64_t* acc_full = bars + 2 * kGemmStages;       // [2]
-  uint64_t* acc_empty = acc_full + 2;                // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_stats = reinterpret_cast<float*>(bars + 16);  // [4][2*NT] (one row per TMEM lane quarter)
+  float* s_stats = reinterpret_cast<float*>(bars + 16);  // [4][2*NT] (one row per 32-row quarter of the tile)
+  float* s_stage = s_stats + 4 * 2 * NT;                 // [2 warpgroups][2][kStageFloats]
 
   const b200_gemm_tc_desc& d = p.d;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform for ptxas
   const int num_k16 = d.K / 16;
   const int num_stages = (num_k16 + kGemmK16PerStage - 1) / kGemmK16PerStage;
   const int n_tiles = d.N / NT, row_tiles = (d.S + 127) / 128;
   const long long total_tiles = (long long)d.Nb * row_tiles * n_tiles;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kGemmStages; ++i) { tc::mbar_init(&full[i], 1); tc::mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&acc_full[i], 1); tc::mbar_init(&acc_empty[i], kGemmEpiWarps); }
+    for (int i = 0; i < kGemmStages; ++i) { tc::mbar_init(&full[i], 1); tc::mbar_init(&empty[i], 2); }
     tc::fence_barrier_init();
   }
   if (STATS)
     for (int i = threadIdx.x; i < 4 * 2 * NT; i += blockDim.x) s_stats[i] = 0.f;
-  if (warp == 1) tc::tmem_alloc(tmem_slot, p.tmem_cols);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -121,7 +129,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(GemmTcParams p
       for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         int nt, rt, n;
         gemm_tile<STATS>(tile, n_tiles, row_tiles, nt, rt, n);
-        const __half* wbase = p.w + (long long)nt * num_k16 * (NT * 16);
+        // the NT columns of this tile inside the packed image of width P: per K16 step two runs (k halves) of NT rows x 16 B
+        const int col = nt * NT, ptile = col / p.P, pcol = col - ptile * p.P;
+        const __half* wbase = p.w + (long long)ptile * num_k16 * (p.P * 16) + pcol * 8;
         for (int st = 0; st < num_stages; ++st) {
           const int steps = min(kGemmK16PerStage, num_k16 - st * kGemmK16PerStage);
           tc::mbar_wait(&empty[s], ph ^ 1);
@@ -132,208 +142,156 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(GemmTcParams p
           const __half* abase = p.x + (((long long)n * (d.in_ctot / 8) + d.in_coff / 8 + st * kGemmK16PerStage * 2) * d.S + rt * 128) * 8;
           for (int c = 0; c < steps * 2; ++c)
             tc::bulk_load(smem_a + s * kGemmAStage + c * 2048, abase + (long long)c * d.S * 8, rows * 16, &full[s]);
-          tc::bulk_load(smem_b + s * b_stage, wbase + (long long)st * kGemmK16PerStage * (NT * 16), steps * NT * 32, &full[s]);
-          if (++s == kGemmStages) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // the whole warp runs the loop control (converged: descriptors stay on the uniform datapath), one elected lane issues
-    {
-      const bool leader = tc::elect_one();
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-      const uint32_t idesc = tc::make_idesc_f16(128, NT);
-      int s = 0; uint32_t ph = 0;
-      int it = 0;
-      for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-        const int buf = it & 1;
-        const uint32_t aph = (uint32_t)((it >> 1) & 1);
-        tc::mbar_wait(&acc_empty[buf], aph ^ 1);     // epilogue has drained this accumulator buffer
-        tc::fence_after_sync();
-        const uint32_t tacc = tmem_u + buf * NT;
-        for (int st = 0; st < num_stages; ++st) {
-          const int steps = min(kGemmK16PerStage, num_k16 - st * kGemmK16PerStage);
-          tc::mbar_wait(&full[s], ph);
-          tc::fence_after_sync();
-          const uint32_t a_base = tc::smem_u32(smem_a + s * kGemmAStage), b_base = tc::smem_u32(smem_b + s * b_stage);
-          for (int k = 0; k < steps; ++k) {
-            const uint64_t adesc = tc::make_desc_kmajor_noswz(a_base + k * 2 * 2048, 2048, 128);
-            const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_base + k * NT * 32, NT * 16, 128);
-            if (leader) tc::mma_f16_ss(tacc, adesc, bdesc, idesc, (st | k) != 0 ? 1u : 0u);
+          const __half* wst = wbase + (long long)st * kGemmK16PerStage * (p.P * 16);
+          if (p.P == NT) {
+            tc::bulk_load(smem_b + s * b_stage, wst, steps * NT * 32, &full[s]);
+          } else {
+            for (int k = 0; k < steps; ++k)
+              for (int kh = 0; kh < 2; ++kh)
+                tc::bulk_load(smem_b + s * b_stage + (k * 2 + kh) * NT * 16, wst + (long long)k * (p.P * 16) + kh * (p.P * 8), NT * 16, &full[s]);
           }
-          if (leader) tc::mma_commit(&empty[s]);
-          __syncwarp();
           if (++s == kGemmStages) { s = 0; ph ^= 1; }
         }
-        if (leader) tc::mma_commit(&acc_full[buf]);
-        __syncwarp();
       }
     }
     __syncwarp();
-  } else {
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int cpart = (warp - 2) >> 2;      // warps sharing a quarter split the 16-column steps between them
+  } else if (warp >= 4) {
+    const int g = (warp >> 2) - 1;          // consumer warpgroup: rows 64 g .. 64 g + 63 of the tile
+    const int wid = warp & 3;
+    const int q = 2 * g + (wid & 1);        // 32-row quarter of the tile this warp writes
+    const int half = wid >> 1;              // which 8 columns of each 16-column slice this warp writes
     const int cout = MODE == 2 ? d.N / 8 : d.N;  // channels of the destination tensor written by this GEMM
-    constexpr int kParts = kGemmEpiWarps / 4;
-    const int n16 = NT / 16, c_lo = (cpart * n16) / kParts, c_hi = ((cpart + 1) * n16) / kParts;
     const long long cs = (long long)d.S_out * 8;   // halves between consecutive 8-channel chunks of the destination
     const float* __restrict__ bias = p.bias;
     const bool has_bias = bias != nullptr;
     const int W2 = 2 * d.W, HW4 = 4 * d.H * d.W;
-    float* ws = s_stats + q * (2 * NT);   // running column sums of this lane quarter; the warps of a quarter own disjoint columns
+    float* ws = s_stats + q * (2 * NT);     // running column sums of this quarter; the two warps of a quarter own disjoint columns
+    float* stage = s_stage + g * 2 * tc::kStageFloats;
     long long group = -1;
-    int it = 0;
-    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+    int s = 0; uint32_t ph = 0;
+    int sl = 0;                             // slice counter: alternates the two slice buffers
+    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int nt, rt, n;
       gemm_tile<STATS>(tile, n_tiles, row_tiles, nt, rt, n);
       if (STATS) {
-        const long long g = tile / row_tiles;   // (batch item, N tile): tiles of a group are contiguous (row tile fastest)
-        if (g != group) {
-          if (group >= 0) stats_flush(p.sp, ws, 2 * NT, group, q, lane, c_lo * 16, c_hi * 16);
-          group = g;
+        const long long gg = tile / row_tiles;   // (batch item, N tile): tiles of a group are contiguous (row tile fastest)
+        if (gg != group) {
+          if (group >= 0) {
+            tc::wg_bar(8 + g);
+            if (half == 0) stats_flush(p.sp, ws, 2 * NT, group, q, lane, 0, NT);
+          }
+          group = gg;
         }
       }
-      const int buf = it & 1;
-      const uint32_t aph = (uint32_t)((it >> 1) & 1);
+      float acc[NT / 2];
+      for (int st = 0; st < num_stages; ++st) {
+        const int steps = min(kGemmK16PerStage, num_k16 - st * kGemmK16PerStage);
+        tc::mbar_wait(&full[s], ph);
+        const uint32_t a_base = tc::smem_u32(smem_a + s * kGemmAStage) + g * 1024, b_base = tc::smem_u32(smem_b + s * b_stage);
+        tc::wg_fence();
+        for (int k = 0; k < steps; ++k) {
+          const uint64_t adesc = tc::make_desc_kmajor_noswz(a_base + k * 2 * 2048, 2048, 128);
+          const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_base + k * NT * 32, NT * 16, 128);
+          tc::wg_mma_ss<NT>(acc, adesc, bdesc, (st | k) != 0 ? 1u : 0u, 128);
+        }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        tc::wg_fence_acc<NT / 2>(acc);
+        if (wid == 0 && lane == 0) tc::mbar_arrive(&empty[s]);
+        if (++s == kGemmStages) { s = 0; ph ^= 1; }
+      }
+
       const int row = rt * 128 + q * 32 + lane;
       const bool row_ok = row < d.S;
       long long drow = row;
       if (MODE == 1) drow = row_ok ? (long long)__ldg(p.row_map + row) : -1;  // the map is shared by all batch items
       const bool dst_ok = row_ok && drow >= 0;
       const int co0 = nt * NT;
-      // running (tap, channel) position of this warp's first column for the upsample scatter
-      int tap = 0, cc = co0 + c_lo * 16;
       if (MODE == 2) {
         const int vx = row % d.W, vy = (row / d.W) % d.H, vz = row / (d.W * d.H);
         drow = ((long long)(2 * vz) * (2 * d.H) + 2 * vy) * W2 + 2 * vx;
-        tap = cc / cout;  // GEMM columns are ordered [tap][cout]
-        cc -= tap * cout;
       }
       __half* ytile = p.y + ((long long)n * (d.out_ctot / 8) + (MODE == 2 ? 0 : (d.out_coff + co0) / 8)) * cs + drow * 8;
       const __half* rtile = RES ? p.res + ((long long)n * (d.res_ctot / 8) + (d.res_coff + co0) / 8) * cs + drow * 8 : nullptr;
-      uint32_t va[16], vb[16];
-      uint4 ra0 = make_uint4(0, 0, 0, 0), ra1 = ra0, rb0 = ra0, rb1 = ra0;
-      // the residual of the first step does not depend on the accumulator: fetch it before waiting for the MMAs
-      if (RES && dst_ok && c_lo < c_hi) {
-        ra0 = *reinterpret_cast<const uint4*>(rtile + (long long)(2 * c_lo) * cs);
-        ra1 = *reinterpret_cast<const uint4*>(rtile + (long long)(2 * c_lo + 1) * cs);
-      }
-      tc::mbar_wait(&acc_full[buf], aph);
-      tc::fence_after_sync();
-      const uint32_t tacc = tmem_base + buf * NT + ((uint32_t)(q * 32) << 16);
-
-      auto process = [&](uint32_t (&v)[16], const uint4& r0, const uint4& r1, int c16) {
-        float f[16];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]);
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          float* g = f + hh * 8;
-          const int g8 = c16 * 2 + hh;           // 8-column group inside this N tile
-          __half* yp;
-          int bidx;
-          if (MODE == 2) {
-            const int tapoff = (tap >> 2) * HW4 + ((tap >> 1) & 1) * W2 + (tap & 1);
-            yp = ytile + (long long)((d.out_coff + cc) >> 3) * cs + (long long)tapoff * 8;
-            bidx = cc;
-            cc += 8;
-            if (cc >= cout) { cc = 0; ++tap; }
-          } else {
-            yp = ytile + (long long)g8 * cs;
-            bidx = co0 + g8 * 8;
-          }
-          if (has_bias) {
-            const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + bidx)), b1 = __ldg(reinterpret_cast<const float4*>(bias + bidx + 4));
-            g[0] += b0.x; g[1] += b0.y; g[2] += b0.z; g[3] += b0.w;
-            g[4] += b1.x; g[5] += b1.y; g[6] += b1.z; g[7] += b1.w;
-          }
-          if (ACT == 4) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) g[j] = gelu_erf(g[j]);
-          }
-          if (RES) {
-            const __half2* rh = reinterpret_cast<const __half2*>(hh ? &r1 : &r0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { const float2 r2 = __half22float2(rh[j]); g[2 * j] += r2.x; g[2 * j + 1] += r2.y; }
-          }
-          if (dst_ok) {
-            uint4 hv;
-            __half2* hp = reinterpret_cast<__half2*>(&hv);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) hp[j] = __floats2half2_rn(g[2 * j], g[2 * j + 1]);
-            *reinterpret_cast<uint4*>(yp) = hv;
-          }
-          if (STATS) {
-            float a8[8], b8[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { a8[j] = dst_ok ? g[j] : 0.f; b8[j] = a8[j] * a8[j]; }
-            float cs, cq;
-            transpose_reduce8(a8, b8, lane, cs, cq);
-            if ((lane & 3) == 0) {
-              const int col = g8 * 8 + transpose_reduce8_col(lane);
-              ws[2 * col] += cs;
-              ws[2 * col + 1] += cq;
-            }
-          }
+      for (int c16 = 0; c16 < NT / 16; ++c16, ++sl) {
+        float* buf = stage + (sl & 1) * tc::kStageFloats;
+        tc::wg_stage16<0>(acc + c16 * 8, buf, wid, lane);
+        tc::wg_bar(8 + g);
+        float gv[8];
+        tc::wg_read8(buf, wid, lane, gv);
+        const int g8 = c16 * 2 + half;           // 8-column group inside this N tile
+        __half* yp;
+        int bidx;
+        if (MODE == 2) {
+          const int col = co0 + g8 * 8;          // GEMM columns are ordered [tap][cout]
+          const int tap = col / cout, cc = col - tap * cout;
+          const int tapoff = (tap >> 2) * HW4 + ((tap >> 1) & 1) * W2 + (tap & 1);
+          yp = ytile + (long long)((d.out_coff + cc) >> 3) * cs + (long long)tapoff * 8;
+          bidx = cc;
+        } else {
+          yp = ytile + (long long)g8 * cs;
+          bidx = co0 + g8 * 8;
         }
-      };
-
-      // 16 columns per step: tcgen05.ld.x16 and the residual are fetched one step ahead into the other register set
-      if (c_lo < c_hi) tc::tmem_ld16(tacc + c_lo * 16, va);
-#pragma unroll 1
-      for (int c16 = c_lo; c16 < c_hi; c16 += 2) {
-        tmem_ld_wait16(va);
-        const bool more = c16 + 1 < c_hi;
-        if (more) {
-          tc::tmem_ld16(tacc + (c16 + 1) * 16, vb);
-          if (RES && dst_ok) {
-            rb0 = *reinterpret_cast<const uint4*>(rtile + (long long)(2 * c16 + 2) * cs);
-            rb1 = *reinterpret_cast<const uint4*>(rtile + (long long)(2 * c16 + 3) * cs);
-          }
+        if (has_bias) {
+          const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + bidx)), b1 = __ldg(reinterpret_cast<const float4*>(bias + bidx + 4));
+          gv[0] += b0.x; gv[1] += b0.y; gv[2] += b0.z; gv[3] += b0.w;
+          gv[4] += b1.x; gv[5] += b1.y; gv[6] += b1.z; gv[7] += b1.w;
         }
-        process(va, ra0, ra1, c16);
-        if (more) {
-          tmem_ld_wait16(vb);
-          if (c16 + 2 < c_hi) {
-            tc::tmem_ld16(tacc + (c16 + 2) * 16, va);
-            if (RES && dst_ok) {
-              ra0 = *reinterpret_cast<const uint4*>(rtile + (long long)(2 * c16 + 4) * cs);
-              ra1 = *reinterpret_cast<const uint4*>(rtile + (long long)(2 * c16 + 5) * cs);
-            }
+        if (ACT == 4) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) gv[j] = gelu_erf(gv[j]);
+        }
+        if (RES) {
+          uint4 r = make_uint4(0, 0, 0, 0);
+          if (dst_ok) r = *reinterpret_cast<const uint4*>(rtile + (long long)g8 * cs);
+          const __half2* rh = reinterpret_cast<const __half2*>(&r);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) { const float2 r2 = __half22float2(rh[j]); gv[2 * j] += r2.x; gv[2 * j + 1] += r2.y; }
+        }
+        if (dst_ok) {
+          uint4 hv;
+          __half2* hp = reinterpret_cast<__half2*>(&hv);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) hp[j] = __floats2half2_rn(gv[2 * j], gv[2 * j + 1]);
+          *reinterpret_cast<uint4*>(yp) = hv;
+        }
+        if (STATS) {
+          float a8[8], b8[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) { a8[j] = dst_ok ? gv[j] : 0.f; b8[j] = a8[j] * a8[j]; }
+          float csum, cq;
+          transpose_reduce8(a8, b8, lane, csum, cq);
+          if ((lane & 3) == 0) {
+            const int col = g8 * 8 + transpose_reduce8_col(lane);
+            ws[2 * col] += csum;
+            ws[2 * col + 1] += cq;
           }
-          process(vb, rb0, rb1, c16 + 1);
         }
       }
-      // this thread's TMEM reads of the buffer are complete: hand it back to the MMA warp (one arrival per warp: 512 per-thread
-      // arrivals per tile serialise on one shared-memory word)
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&acc_empty[buf]);
     }
-    if (STATS && group >= 0) stats_flush(p.sp, ws, 2 * NT, group, q, lane, c_lo * 16, c_hi * 16);
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, p.tmem_cols);
+    if (STATS && group >= 0) {
+      tc::wg_bar(8 + g);
+      if (half == 0) stats_flush(p.sp, ws, 2 * NT, group, q, lane, 0, NT);
+    }
   }
 }
 
 using GemmKernelFn = void (*)(GemmTcParams);
 
-template <int MODE, int ACT>
+template <int NT, int MODE, int ACT>
 static GemmKernelFn gemm_pick2(bool res, bool stats) {
-  if (res) return stats ? gemm_tc_kernel<MODE, ACT, true, true> : gemm_tc_kernel<MODE, ACT, true, false>;
-  return stats ? gemm_tc_kernel<MODE, ACT, false, true> : gemm_tc_kernel<MODE, ACT, false, false>;
+  if (res) return stats ? gemm_tc_kernel<NT, MODE, ACT, true, true> : gemm_tc_kernel<NT, MODE, ACT, true, false>;
+  return stats ? gemm_tc_kernel<NT, MODE, ACT, false, true> : gemm_tc_kernel<NT, MODE, ACT, false, false>;
 }
 
+template <int NT>
 static GemmKernelFn gemm_pick(int mode, int act, bool res, bool stats) {
-  if (mode == 0) return act == 4 ? gemm_pick2<0, 4>(res, stats) : gemm_pick2<0, 0>(res, stats);
-  if (mode == 1) return act == 4 ? gemm_pick2<1, 4>(res, stats) : gemm_pick2<1, 0>(res, stats);
+  if (mode == 0) return act == 4 ? gemm_pick2<NT, 0, 4>(res, stats) : gemm_pick2<NT, 0, 0>(res, stats);
+  if (mode == 1) return act == 4 ? gemm_pick2<NT, 1, 4>(res, stats) : gemm_pick2<NT, 1, 0>(res, stats);
   if (res) return nullptr;  // the upsample scatter has no residual form
-  if (act == 4) return stats ? gemm_tc_kernel<2, 4, false, true> : gemm_tc_kernel<2, 4, false, false>;
-  return stats ? gemm_tc_kernel<2, 0, false, true> : gemm_tc_kernel<2, 0, false, false>;
+  if (act == 4) return stats ? gemm_tc_kernel<NT, 2, 4, false, true> : gemm_tc_kernel<NT, 2, 4, false, false>;
+  return stats ? gemm_tc_kernel<NT, 2, 0, false, true> : gemm_tc_kernel<NT, 2, 0, false, false>;
 }
 
 }  // namespace b200
@@ -373,7 +331,7 @@ static int gemm_tc_check(const b200_gemm_tc_desc& d, const void* res, const int3
 
 extern "C" long long b200_gemm_tc_workspace_bytes(const b200_gemm_tc_desc* desc) {
   if (!desc || desc->N <= 0 || desc->N % 16 || desc->S <= 0 || desc->Nb <= 0) return -1;
-  const int NT = gemm_tc_nt(desc->N);
+  const int NT = gemm_tile_n(gemm_tc_nt(desc->N));   // the kernel's N tile: one statistics group per (batch item, N tile)
   const long long row_tiles = ceil_div(desc->S, 128), groups = (long long)desc->Nb * (desc->N / NT);
   return stats_partial_bytes(groups, stats_rows(row_tiles, row_tiles * groups), NT);
 }
@@ -385,15 +343,23 @@ extern "C" int b200_gemm_tc(const b200_gemm_tc_desc* desc, const void* x, const 
   const b200_gemm_tc_desc& d = *desc;
   int rc = gemm_tc_check(d, res, row_map);
   if (rc) return rc;
-  const int NT = gemm_tc_nt(d.N);
+  const int P = gemm_tc_nt(d.N), NT = gemm_tile_n(P);
   GemmTcParams p;
   p.d = d; p.x = (const __half*)x; p.w = (const __half*)packed_w; p.bias = bias; p.y = (__half*)y; p.res = (const __half*)res;
-  p.row_map = row_map; p.NT = NT;
-  p.tmem_cols = 2 * NT <= 32 ? 32 : 2 * NT <= 64 ? 64 : 2 * NT <= 128 ? 128 : 2 * NT <= 256 ? 256 : 512;  // two accumulator buffers
-  const int smem = kGemmStages * (kGemmAStage + kGemmK16PerStage * NT * 32) + 128 + 4 * 2 * NT * 4 + 128;
-  GemmKernelFn fn = gemm_pick(d.mode, d.act, res != nullptr, stats != nullptr);
+  p.row_map = row_map; p.P = P;
+  int smem = 0;
+  GemmKernelFn fn = nullptr;
+  const bool has_res = res != nullptr, has_stats = stats != nullptr;
+  switch (NT) {
+    case 128: fn = gemm_pick<128>(d.mode, d.act, has_res, has_stats); smem = gemm_smem_bytes<128>(); break;
+    case 96: fn = gemm_pick<96>(d.mode, d.act, has_res, has_stats); smem = gemm_smem_bytes<96>(); break;
+    case 64: fn = gemm_pick<64>(d.mode, d.act, has_res, has_stats); smem = gemm_smem_bytes<64>(); break;
+    case 48: fn = gemm_pick<48>(d.mode, d.act, has_res, has_stats); smem = gemm_smem_bytes<48>(); break;
+    case 32: fn = gemm_pick<32>(d.mode, d.act, has_res, has_stats); smem = gemm_smem_bytes<32>(); break;
+    default: fn = gemm_pick<16>(d.mode, d.act, has_res, has_stats); smem = gemm_smem_bytes<16>(); break;
+  }
   B200_REQUIRE(fn != nullptr, "gemm_tc: the 2x upsample scatter (mode 2) does not take a residual");
-  B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const long long row_tiles = ceil_div(d.S, 128), groups = (long long)d.Nb * (d.N / NT);
   const long long total_tiles = row_tiles * groups;
   p.sp.buf = stats ? (float*)workspace : nullptr;

@@ -1,21 +1,21 @@
-// Output head on tcgen05 tensor cores (SURVEY.md §8 rows a9, a14): the tail of the last residual block fused with UnetOutBlock,
+// Output head on Hopper wgmma tensor cores (SURVEY.md §8 rows a9, a14): the tail of the last residual block fused with UnetOutBlock,
 //     logits = W_out * lrelu(instnorm(y2) + instnorm(res)) + b_out
 // (monai/networks/blocks/dynunet_block.py:104-111 followed by 247-267: norm2 + residual (norm3 of the 1x1x1 branch, or the block
 // input) + LeakyReLU, then the 1x1x1 convolution to <= 16 classes) for C = 48 input channels.
 //
 // Why: the CUDA-core version (swin.cu: head_conv_norm_nc8_kernel) spends 2 100 instructions per voxel -- 14 x 48 FMAs plus the
 // weight reads -- and runs at 1.8 TB/s (ncu: 49 % issue-active with 24 resident warps).  Here the 48 -> 16 contraction is one
-// UMMA (M = 128 voxels, N = 16, K = 48) and the threads only normalise: per 128-voxel tile
+// MMA (M = 128 voxels, N = 16, K = 48) and the threads only normalise: per 128-voxel tile
 //   bulk copies of the y2 and residual tiles (NC8 rows: 2 KB per 8-channel chunk)  ->  t = lrelu(y2 * sc + sh + res * rsc + rsh),
-//   fp16, written in place over the y2 tile = the K-major core-matrix image of the A operand  ->  UMMA into TMEM  ->
+//   fp16, written in place over the y2 tile = the K-major core-matrix image of the A operand  ->  wgmma into registers  ->
 //   + bias  ->  NCDHW logits (fp16 / fp32).
 // The per-(batch item, channel) scale / shift tables of ALL batch items are built once per CTA in shared memory.
 //
-// Warp roles (320 threads, one persistent CTA per SM): warp 0 = copy producer, warp 1 = TMEM owner + MMA issuer, warps 2-5 and
-// 6-9 = two "row" groups that alternate tiles (transform of tile i, then the output of tile i - 2 of the same group); four
-// operand stages keep ~96 KB of loads in flight per SM.
+// Warp roles (384 threads, one persistent CTA per SM): warp 0 = copy producer, warps 4-7 and 8-11 = two "row" warpgroups that
+// alternate tiles (transform of the tile, its two m64 wgmma chains, output); four operand stages keep ~96 KB of loads in
+// flight per SM.
 #include "common.cuh"
-#include "tc05.cuh"
+#include "tc90.cuh"
 #include "../../include/monai_b200.h"
 
 namespace b200 {
@@ -35,7 +35,7 @@ struct HeadTcParams {
 };
 
 template <typename TO>
-__global__ void __launch_bounds__(320, 1) head_conv_norm_tc_kernel(HeadTcParams p) {
+__global__ void __launch_bounds__(384, 1) head_conv_norm_tc_kernel(HeadTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = tc::align_smem128(smem_raw);
   uint8_t* s_x = smem;                                  // [kHdStages] y2 tiles (raw, then t in place)
@@ -43,21 +43,17 @@ __global__ void __launch_bounds__(320, 1) head_conv_norm_tc_kernel(HeadTcParams 
   uint8_t* s_w = s_r + kHdStages * kHdTile;             // B image of W_out (16 x 48)
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_w + kHdWBytes);
   uint64_t* x_full = bars;                      // [kHdStages] tx
-  uint64_t* x_free = bars + kHdStages;          // [kHdStages] commit
-  uint64_t* a_ready = bars + 2 * kHdStages;     // [kHdStages] 128 arrivals
-  uint64_t* d_full = bars + 3 * kHdStages;      // [2] commit
-  uint64_t* d_free = d_full + 2;                // [2] 128 arrivals
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d_free + 2);
+  uint64_t* x_free = bars + kHdStages;          // [kHdStages] one arrival: the MMAs of the stage have completed
   float* s_bias = reinterpret_cast<float*>(bars + 3 * kHdStages + 6);  // [16]
-  float4* s_tab = reinterpret_cast<float4*>(s_bias + 16);   // [N][48] {sc, sh, rsc, rsh}
+  float* s_out = s_bias + 16;                   // [2 row groups][16 cout][128 rows] accumulator transpose
+  float4* s_tab = reinterpret_cast<float4*>(s_out + 2 * 16 * 128);   // [N][48] {sc, sh, rsc, rsh}
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int row_tiles = (int)((p.S + 127) / 128);
   const long long total = (long long)p.N * row_tiles;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kHdStages; ++i) { tc::mbar_init(&x_full[i], 1); tc::mbar_init(&x_free[i], 1); tc::mbar_init(&a_ready[i], 128); }
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&d_full[i], 1); tc::mbar_init(&d_free[i], 128); }
+    for (int i = 0; i < kHdStages; ++i) { tc::mbar_init(&x_full[i], 1); tc::mbar_init(&x_free[i], 1); }
     tc::fence_barrier_init();
   }
   {  // rows a clamped bulk copy never writes must hold finite values
@@ -92,12 +88,8 @@ __global__ void __launch_bounds__(320, 1) head_conv_norm_tc_kernel(HeadTcParams 
       s_tab[i] = t;
     }
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, 32);
   tc::fence_proxy_async();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ===================== producer =====================
@@ -119,57 +111,18 @@ __global__ void __launch_bounds__(320, 1) head_conv_norm_tc_kernel(HeadTcParams 
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const bool leader = tc::elect_one();
-    const uint32_t tm = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const uint32_t idesc = tc::make_idesc_f16(128, kHdN);
-    const uint32_t x_a = tc::smem_u32(s_x), w_a = tc::smem_u32(s_w);
-    int it = 0;
-    for (long long t = blockIdx.x; t < total; t += gridDim.x, ++it) {
-      const int st = it % kHdStages, b = it & 1;
-      tc::mbar_wait(&a_ready[st], (uint32_t)((it / kHdStages) & 1));
-      tc::mbar_wait(&d_free[b], (uint32_t)(((it >> 1) & 1) ^ 1));
-      tc::fence_after_sync();
-#pragma unroll
-      for (int k = 0; k < kHdC / 16; ++k) {
-        const uint64_t ad = tc::make_desc_kmajor_noswz(x_a + st * kHdTile + k * 4096, 2048, 128);
-        const uint64_t bd = tc::make_desc_kmajor_noswz(w_a + k * kHdN * 32, kHdN * 16, 128);
-        if (leader) tc::mma_f16_ss(tm + b * kHdN, ad, bd, idesc, k != 0 ? 1u : 0u);
-      }
-      if (leader) { tc::mma_commit(&d_full[b]); tc::mma_commit(&x_free[st]); }
-      __syncwarp();
-    }
-    __syncwarp();
-  } else {
-    // ===================== row groups: group g = stage g: transform of its tile, then the output of its previous tile =====================
-    const int g = (warp - 2) >> 2;            // 0 / 1 = stage = tile parity
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
+  } else if (warp >= 4) {
+    // ===================== row groups: group g (a warpgroup) takes every other tile: transform, MMA, output =====================
+    const int g = (warp >> 2) - 1;            // 0 / 1 = tile parity
+    const int wid = warp & 3;
+    const int row = wid * 32 + lane;
     const float slope = p.slope;
-    auto output = [&](int it, long long t) {
-      const uint32_t ph = (uint32_t)((it >> 1) & 1);
-      const int n = (int)(t / row_tiles), rt = (int)(t % row_tiles);
-      const long long r = (long long)rt * 128 + row;
-      tc::mbar_wait(&d_full[g], ph);
-      tc::fence_after_sync();
-      uint32_t v[16];
-      tc::tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + g * kHdN, v);
-      tc::tmem_ld_wait16(v);
-      tc::fence_before_sync();
-      tc::mbar_arrive(&d_free[g]);
-      if (r < p.S) {
-        TO* yo = (TO*)p.y + (long long)n * p.Cout * p.S + r;
-#pragma unroll
-        for (int o = 0; o < 16; ++o)
-          if (o < p.Cout) io<TO>::st(yo + (long long)o * p.S, __uint_as_float(v[o]) + s_bias[o]);
-      }
-    };
+    const uint32_t x_a = tc::smem_u32(s_x), w_a = tc::smem_u32(s_w);
+    float* so = s_out + g * 16 * 128;
     int it = g;
-    long long prev_t = -1;
     for (long long t = (long long)blockIdx.x + (long long)g * gridDim.x; t < total; t += 2LL * gridDim.x, it += 2) {
       const int st = it % kHdStages;
-      const int n = (int)(t / row_tiles);
+      const int n = (int)(t / row_tiles), rt = (int)(t % row_tiles);
       tc::mbar_wait(&x_full[st], (uint32_t)((it / kHdStages) & 1));
       uint8_t* xr = s_x + st * kHdTile + row * 16;
       const uint8_t* rr = s_r + st * kHdTile + row * 16;
@@ -193,17 +146,43 @@ __global__ void __launch_bounds__(320, 1) head_conv_norm_tc_kernel(HeadTcParams 
         }
         *reinterpret_cast<uint4*>(xr + c * 2048) = o;
       }
-      tc::fence_proxy_async();
-      tc::mbar_arrive(&a_ready[st]);
-      if (prev_t >= 0) output(it - 2, prev_t);
-      prev_t = t;
+      tc::fence_proxy_async();   // generic-proxy stores -> visible to the wgmma operand reads
+      tc::wg_bar(8 + g);         // the whole 128-row A image is written (and the previous tile's s_out reads are done)
+      float acc[2][kHdN / 2];
+      tc::wg_fence();
+#pragma unroll
+      for (int k = 0; k < kHdC / 16; ++k) {
+        const uint64_t bd = tc::make_desc_kmajor_noswz(w_a + k * kHdN * 32, kHdN * 16, 128);
+#pragma unroll
+        for (int m = 0; m < 2; ++m) {
+          const uint64_t ad = tc::make_desc_kmajor_noswz(x_a + st * kHdTile + k * 4096 + m * 1024, 2048, 128);
+          tc::wg_mma_ss<kHdN>(acc[m], ad, bd, k != 0 ? 1u : 0u, 128);
+        }
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc<kHdN / 2>(acc[0]);
+      tc::wg_fence_acc<kHdN / 2>(acc[1]);
+      if (wid == 0 && lane == 0) tc::mbar_arrive(&x_free[st]);
+      // fragment (rows 64 m + 16 wid + lane/4 (+8), columns 8 i + 2 (lane%4) (+1)) -> [cout][row] -> one row per thread
+#pragma unroll
+      for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int i = 0; i < kHdN / 8; ++i)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int r = 64 * m + 16 * wid + (lane >> 2) + 8 * (e >> 1), c = 8 * i + 2 * (lane & 3) + (e & 1);
+            so[c * 128 + r] = acc[m][4 * i + e];
+          }
+      tc::wg_bar(8 + g);
+      const long long r = (long long)rt * 128 + row;
+      if (r < p.S) {
+        TO* yo = (TO*)p.y + (long long)n * p.Cout * p.S + r;
+#pragma unroll
+        for (int o = 0; o < 16; ++o)
+          if (o < p.Cout) io<TO>::st(yo + (long long)o * p.S, so[o * 128 + row] + s_bias[o]);
+      }
     }
-    if (prev_t >= 0) output(it - 2, prev_t);
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, 32);
   }
 }
 
@@ -213,15 +192,15 @@ int launch_head_conv_norm_tc(const void* x, int N, int C, long long S, const flo
                              void* y, int out_dtype, cudaStream_t st) {
   if (C != kHdC || !res || (long long)N * C * 16 > kHdMaxTab || Cout > 16) return B200_ERR_UNSUPPORTED;
   HeadTcParams p{(const __half*)x, (const __half*)res, stats, res_stats, weight, bias, y, N, Cout, res_ctot, res_coff, S, eps, slope};
-  const int smem = 2 * kHdStages * kHdTile + kHdWBytes + (3 * kHdStages + 6) * 8 + 64 + N * C * 16 + 128;
+  const int smem = 2 * kHdStages * kHdTile + kHdWBytes + (3 * kHdStages + 6) * 8 + 64 + 2 * 16 * 128 * 4 + N * C * 16 + 128;
   const long long total = (long long)N * ((S + 127) / 128);
   dim3 grid((unsigned)std::min<long long>(total, num_sms()));
   if (out_dtype == B200_DT_F16) {
     B200_CUDA(cudaFuncSetAttribute(head_conv_norm_tc_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    head_conv_norm_tc_kernel<__half><<<grid, 320, smem, st>>>(p);
+    head_conv_norm_tc_kernel<__half><<<grid, 384, smem, st>>>(p);
   } else {
     B200_CUDA(cudaFuncSetAttribute(head_conv_norm_tc_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    head_conv_norm_tc_kernel<float><<<grid, 320, smem, st>>>(p);
+    head_conv_norm_tc_kernel<float><<<grid, 384, smem, st>>>(p);
   }
   B200_LAUNCH_CHECK("head_conv_norm_tc_kernel");
   return B200_OK;

@@ -29,7 +29,7 @@ int num_sms() {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached = n;
     else
-      cached = 148;
+      cached = 132;   // H100 SXM
   }
   return cached;
 }

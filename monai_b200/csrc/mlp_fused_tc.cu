@@ -1,24 +1,21 @@
-// Fused transformer MLP on tcgen05 tensor cores (SURVEY.md §8 rows a12, a13):
+// Fused transformer MLP on Hopper wgmma tensor cores (SURVEY.md §8 rows a12, a13):
 //     out = x + W2 * gelu(W1 * LayerNorm(x) + b1) + b2
 // i.e. norm2 + MLPBlock + the residual add of SwinTransformerBlock.forward (monai/networks/nets/swin_unetr.py:675-698 with
-// monai/networks/blocks/mlp.py:75-80) in ONE kernel for C = 48 tokens (stage 1 of SwinUNETR fs48: 82 % of the MLP time).
+// monai/networks/blocks/mlp.py:75-80) in ONE kernel for C = 48 tokens (stage 1 of SwinUNETR fs48).
 //
 // Why: as separate launches the 4C-wide hidden tensor is written by fc1 and read again by fc2 (768 of the 1 344 bytes the MLP
 // moves per token) and LayerNorm is a pass of its own.  Here a 128-token tile flows through
 //   bulk copy X (NC8 rows: one contiguous 2 KB piece per 8-channel chunk)  ->  LayerNorm in place in shared memory (a thread
-//   per token)  ->  GEMM1 [128 x 48] x W1^T into TMEM (192 fp32 columns)  ->  + b1, GELU, fp16, written straight into the
-//   K-major core-matrix image of the next A operand  ->  GEMM2 [128 x 192] x W2^T into TMEM (48 columns)  ->  + b2 + x  ->  NC8.
-// Both weight matrices (2 x 18 KB as UMMA B images, the same packing as gemm_tc.cu) stay resident in shared memory; the hidden
-// activations never leave the SM.  What is left is bound by the GELU polynomial on the FP32 pipe (~15 FMA-pipe operations per
-// hidden element), not by memory.
+//   per token)  ->  GEMM1 [64 x 48] x W1^T per warpgroup into registers (192 fp32 columns)  ->  + b1, GELU, fp16 -- the
+//   accumulator fragment of GEMM1 IS the register A operand of GEMM2 (same row / column ownership), so the hidden activations
+//   never leave the registers  ->  GEMM2 [64 x 192] x W2^T (48 columns)  ->  + b2 + x  ->  NC8.
+// Both weight matrices (2 x 18 KB as wgmma B images, the same packing as gemm_tc.cu) stay resident in shared memory.
 //
-// Warp roles (704 threads, one persistent CTA per SM):
+// Warp roles (384 threads, one persistent CTA per SM):
 //   warp 0      producer: weights once, then one X tile per iteration (2-stage ring);
-//   warp 1      TMEM owner + MMA issuer; GEMM1 of tile t+1 is issued before GEMM2 of tile t (software pipeline);
-//   warps 2-5   "row" warps: LayerNorm of tile t+1, then the output epilogue of tile t;
-//   warps 6-21  GELU warps: four per TMEM lane quarter, 48 hidden columns each.
+//   warps 4-11  two consumer warpgroups, rows 0-63 / 64-127 of every tile: LayerNorm, GEMM1, GELU, GEMM2, epilogue.
 #include "common.cuh"
-#include "tc05.cuh"
+#include "tc90.cuh"
 #include "gelu.cuh"
 #include "../../include/monai_b200.h"
 
@@ -26,12 +23,10 @@ namespace b200 {
 
 constexpr int kMlpC = 48, kMlpH = 192;
 constexpr int kMlpXBytes = (kMlpC / 8) * 2048;        // one X tile: 6 chunks of 128 rows x 16 B
-constexpr int kMlpHBytes = (kMlpH / 8) * 2048;        // one hidden tile
 constexpr int kMlpW1Bytes = kMlpH * kMlpC * 2, kMlpW2Bytes = kMlpC * kMlpH * 2;
 constexpr int kMlpParFloats = 3 * kMlpC + kMlpH;     // gamma, beta, b2, b1
-constexpr int kMlpSmem = 2 * kMlpXBytes + 2 * kMlpHBytes + kMlpW1Bytes + kMlpW2Bytes + 256 + kMlpParFloats * 4 + 128;
-constexpr int kMlpThreads = 64 + 128 + 512;
-constexpr int kMlpColD2 = 2 * kMlpH;                  // TMEM: D1 buffers at 0 / 192, D2 buffers at 384 / 432
+constexpr int kMlpSmem = 2 * kMlpXBytes + kMlpW1Bytes + kMlpW2Bytes + 256 + kMlpParFloats * 4 + 2 * 2 * tc::kStageFloats * 4 + 128;
+constexpr int kMlpThreads = 384;
 
 struct MlpParams {
   const __half* x; __half* y; const __half* w1; const __half* w2;
@@ -41,58 +36,47 @@ struct MlpParams {
   int x_ctot, y_ctot;   // channel counts of the NC8 buffers (== 48)
 };
 
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+
 __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_tc_kernel(MlpParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = tc::align_smem128(smem_raw);   // keeps the shared address space (LDS/STS, not generic LD/ST)
   uint8_t* s_x = smem;                                  // [2] X tiles (raw, then normalised in place)
-  uint8_t* s_h = s_x + 2 * kMlpXBytes;                  // [2] hidden tiles (A operand of GEMM2)
-  uint8_t* s_w1 = s_h + 2 * kMlpHBytes;
+  uint8_t* s_w1 = s_x + 2 * kMlpXBytes;
   uint8_t* s_w2 = s_w1 + kMlpW1Bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_w2 + kMlpW2Bytes);
   uint64_t* x_full = bars;          // [2] tx
-  uint64_t* x_free = bars + 2;      // [2] commit (GEMM1 has read the tile)
-  uint64_t* ln_done = bars + 4;     // [2] 4 arrivals (one per row warp)
-  uint64_t* d1_full = bars + 6;     // [2] commit
-  uint64_t* d1_free = bars + 8;     // [2] 16 arrivals (one per GELU warp)
-  uint64_t* h_full = bars + 10;     // [2] 16 arrivals
-  uint64_t* h_free = bars + 12;     // [2] commit (GEMM2 has read the tile)
-  uint64_t* d2_full = bars + 14;    // [2] commit
-  uint64_t* d2_free = bars + 16;    // [2] 4 arrivals
-  uint64_t* w_full = bars + 18;     // tx
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 19);
+  uint64_t* x_free = bars + 2;      // [2] one arrival per consumer warpgroup (GEMM1 has read its half of the tile)
+  uint64_t* w_full = bars + 4;      // tx
   float* s_gamma = reinterpret_cast<float*>(bars + 32);   // 256 bytes of barrier space precede the parameter table
   float* s_beta = s_gamma + kMlpC;
   float* s_b2 = s_beta + kMlpC;
   float* s_b1 = s_b2 + kMlpC;
+  float* s_stage = s_b1 + kMlpH;                         // [2 warpgroups][2][kStageFloats]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int row_tiles = (p.S + 127) / 128;
   const long long total = (long long)p.Nb * row_tiles;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&x_full[i], 1); tc::mbar_init(&x_free[i], 1); tc::mbar_init(&ln_done[i], 4);
-      tc::mbar_init(&d1_full[i], 1); tc::mbar_init(&d1_free[i], 16); tc::mbar_init(&h_full[i], 16); tc::mbar_init(&h_free[i], 1);
-      tc::mbar_init(&d2_full[i], 1); tc::mbar_init(&d2_free[i], 4);
-    }
+    for (int i = 0; i < 2; ++i) { tc::mbar_init(&x_full[i], 1); tc::mbar_init(&x_free[i], 2); }
     tc::mbar_init(w_full, 1);
     tc::fence_barrier_init();
   }
   {  // rows a clamped bulk copy never writes must hold finite values
     const uint4 z = make_uint4(0, 0, 0, 0);
     uint4* zx = reinterpret_cast<uint4*>(s_x);
-    for (int i = threadIdx.x; i < (2 * kMlpXBytes + 2 * kMlpHBytes) / 16; i += blockDim.x) zx[i] = z;
+    for (int i = threadIdx.x; i < 2 * kMlpXBytes / 16; i += blockDim.x) zx[i] = z;
   }
   for (int i = threadIdx.x; i < kMlpC; i += blockDim.x) {
     s_gamma[i] = p.gamma ? p.gamma[i] : 1.f; s_beta[i] = p.beta ? p.beta[i] : 0.f; s_b2[i] = p.b2[i];
   }
   for (int i = threadIdx.x; i < kMlpH; i += blockDim.x) s_b1[i] = p.b1[i];
-  if (warp == 1) tc::tmem_alloc(tmem_slot, 512);
   tc::fence_proxy_async();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ===================== producer =====================
@@ -113,181 +97,116 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_tc_kernel(MlpParams 
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const bool leader = tc::elect_one();
-    const uint32_t tm = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const uint32_t idesc1 = tc::make_idesc_f16(128, kMlpH), idesc2 = tc::make_idesc_f16(128, kMlpC);
-    const uint32_t x_a = tc::smem_u32(s_x), h_a = tc::smem_u32(s_h), w1_a = tc::smem_u32(s_w1), w2_a = tc::smem_u32(s_w2);
+  } else if (warp >= 4) {
+    const int g = (warp >> 2) - 1, wid = warp & 3;
+    const uint32_t x_a = tc::smem_u32(s_x), w1_a = tc::smem_u32(s_w1), w2_a = tc::smem_u32(s_w2);
+    float* stage = s_stage + g * 2 * tc::kStageFloats;
+    const int c_lane = 2 * (lane & 3);        // first fragment column of this thread inside each 8-column block
+    int sl = 0;
     tc::mbar_wait(w_full, 0u);
-    auto gemm1 = [&](int it) {   // D1[b] = LN(X)[b] * W1^T
-      const int b = it & 1;
-      const uint32_t ph = (uint32_t)((it >> 1) & 1);
-      tc::mbar_wait(&ln_done[b], ph);
-      tc::mbar_wait(&d1_free[b], ph ^ 1);
-      tc::fence_after_sync();
-#pragma unroll
-      for (int k = 0; k < kMlpC / 16; ++k) {
-        const uint64_t ad = tc::make_desc_kmajor_noswz(x_a + b * kMlpXBytes + k * 4096, 2048, 128);
-        const uint64_t bd = tc::make_desc_kmajor_noswz(w1_a + k * kMlpH * 32, kMlpH * 16, 128);
-        if (leader) tc::mma_f16_ss(tm + b * kMlpH, ad, bd, idesc1, k != 0 ? 1u : 0u);
-      }
-      if (leader) { tc::mma_commit(&d1_full[b]); tc::mma_commit(&x_free[b]); }
-      __syncwarp();
-    };
-    auto gemm2 = [&](int it) {   // D2[b] = gelu(D1)[b] * W2^T
-      const int b = it & 1;
-      const uint32_t ph = (uint32_t)((it >> 1) & 1);
-      tc::mbar_wait(&h_full[b], ph);
-      tc::mbar_wait(&d2_free[b], ph ^ 1);
-      tc::fence_after_sync();
-#pragma unroll
-      for (int k = 0; k < kMlpH / 16; ++k) {
-        const uint64_t ad = tc::make_desc_kmajor_noswz(h_a + b * kMlpHBytes + k * 4096, 2048, 128);
-        const uint64_t bd = tc::make_desc_kmajor_noswz(w2_a + k * kMlpC * 32, kMlpC * 16, 128);
-        if (leader) tc::mma_f16_ss(tm + kMlpColD2 + b * kMlpC, ad, bd, idesc2, k != 0 ? 1u : 0u);
-      }
-      if (leader) { tc::mma_commit(&d2_full[b]); tc::mma_commit(&h_free[b]); }
-      __syncwarp();
-    };
-    long long ntile = 0;
-    for (long long t = blockIdx.x; t < total; t += gridDim.x) ++ntile;
-    if (ntile > 0) gemm1(0);
-    for (int it = 0; it < (int)ntile; ++it) {
-      if (it + 1 < (int)ntile) gemm1(it + 1);
-      gemm2(it);
-    }
-    __syncwarp();
-  } else if (warp < 6) {
-    // ===================== row warps: LayerNorm (one tile ahead) + output epilogue =====================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    auto layer_norm = [&](int it) {
-      const int b = it & 1;
-      const uint32_t ph = (uint32_t)((it >> 1) & 1);
-      tc::mbar_wait(&x_full[b], ph);
-      uint8_t* xr = s_x + b * kMlpXBytes + row * 16;
-      float f[kMlpC];
-#pragma unroll
-      for (int c = 0; c < kMlpC / 8; ++c) {
-        const uint4 raw = *reinterpret_cast<const uint4*>(xr + c * 2048);
-        const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { const float2 v = __half22float2(h2[j]); f[c * 8 + 2 * j] = v.x; f[c * 8 + 2 * j + 1] = v.y; }
-      }
-      float sum = 0.f;
-#pragma unroll
-      for (int c = 0; c < kMlpC; ++c) sum += f[c];
-      const float mean = sum * (1.f / kMlpC);
-      float var = 0.f;
-#pragma unroll
-      for (int c = 0; c < kMlpC; ++c) { const float d = f[c] - mean; var = fmaf(d, d, var); }
-      const float rstd = 1.f / sqrtf(var * (1.f / kMlpC) + p.eps);
-#pragma unroll
-      for (int c = 0; c < kMlpC / 8; ++c) {
-        uint4 o;
-        __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int k = c * 8 + 2 * j;
-          oh[j] = __floats2half2_rn((f[k] - mean) * rstd * s_gamma[k] + s_beta[k], (f[k + 1] - mean) * rstd * s_gamma[k + 1] + s_beta[k + 1]);
-        }
-        *reinterpret_cast<uint4*>(xr + c * 2048) = o;
-      }
-      tc::fence_proxy_async();
-      __syncwarp();                     // one arrival per warp: per-thread arrivals serialise on one shared-memory word
-      if (lane == 0) tc::mbar_arrive(&ln_done[b]);
-    };
-    auto epilogue = [&](int it, long long t) {
+    int it = 0;
+    for (long long t = blockIdx.x; t < total; t += gridDim.x, ++it) {
       const int b = it & 1;
       const uint32_t ph = (uint32_t)((it >> 1) & 1);
       const int n = (int)(t / row_tiles), rt = (int)(t % row_tiles);
-      const int r = rt * 128 + row;
-      const bool ok = r < p.S;
-      // the residual (the raw x row) is re-read from global memory (an L2 hit: the tile was streamed a moment ago)
-      const __half* xg = p.x + ((long long)n * (p.x_ctot / 8) * p.S + r) * 8;
-      uint4 res[kMlpC / 8];
+      tc::mbar_wait(&x_full[b], ph);
+      // ---- LayerNorm of the warpgroup's 64 rows, in place (warps 0-1 of the group, one row per thread) ----
+      if (wid < 2) {
+        uint8_t* xr = s_x + b * kMlpXBytes + (64 * g + 32 * wid + lane) * 16;
+        float f[kMlpC];
 #pragma unroll
-      for (int c = 0; c < kMlpC / 8; ++c) res[c] = ok ? __ldg(reinterpret_cast<const uint4*>(xg + (long long)c * p.S * 8)) : make_uint4(0, 0, 0, 0);
-      tc::mbar_wait(&d2_full[b], ph);
-      tc::fence_after_sync();
-      const uint32_t td = tmem_base + ((uint32_t)(q * 32) << 16) + kMlpColD2 + b * kMlpC;
-      uint32_t v0[16], v1[16], v2[16];
-      tc::tmem_ld16(td, v0); tc::tmem_ld16(td + 16, v1); tc::tmem_ld16(td + 32, v2);
-      tc::tmem_ld_wait16(v0); tc::tmem_ld_wait16(v1); tc::tmem_ld_wait16(v2);
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&d2_free[b]);
-      if (ok) {
-        __half* yg = p.y + ((long long)n * (p.y_ctot / 8) * p.S + r) * 8;
-        auto put = [&](const uint32_t (&v)[16], int c16) {
+        for (int c = 0; c < kMlpC / 8; ++c) {
+          const uint4 raw = *reinterpret_cast<const uint4*>(xr + c * 2048);
+          const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
 #pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            const int c = c16 * 2 + hh;
-            const __half2* rh = reinterpret_cast<const __half2*>(&res[c]);
-            uint4 o;
-            __half2* oh = reinterpret_cast<__half2*>(&o);
+          for (int j = 0; j < 4; ++j) { const float2 v = __half22float2(h2[j]); f[c * 8 + 2 * j] = v.x; f[c * 8 + 2 * j + 1] = v.y; }
+        }
+        float sum = 0.f;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float2 rr = __half22float2(rh[j]);
-              const int k = c * 8 + 2 * j;
-              oh[j] = __floats2half2_rn(__uint_as_float(v[hh * 8 + 2 * j]) + s_b2[k] + rr.x, __uint_as_float(v[hh * 8 + 2 * j + 1]) + s_b2[k + 1] + rr.y);
-            }
-            *reinterpret_cast<uint4*>(yg + (long long)c * p.S * 8) = o;
-          }
-        };
-        put(v0, 0); put(v1, 1); put(v2, 2);
-      }
-    };
-    int it = 0;
-    if ((long long)blockIdx.x < total) layer_norm(0);
-    for (long long t = blockIdx.x; t < total; t += gridDim.x, ++it) {
-      if (t + gridDim.x < total) layer_norm(it + 1);
-      epilogue(it, t);
-    }
-  } else {
-    // ===================== GELU warps: D1 -> + b1 -> gelu -> fp16 H (A operand image of GEMM2) =====================
-    const int q = warp & 3;
-    const int part = (warp - 6) >> 2;              // 0..3: 48 hidden columns each
-    const int row = q * 32 + lane;
-    int it = 0;
-    for (long long t = blockIdx.x; t < total; t += gridDim.x, ++it) {
-      const int b = it & 1;
-      const uint32_t ph = (uint32_t)((it >> 1) & 1);
-      tc::mbar_wait(&d1_full[b], ph);
-      tc::mbar_wait(&h_free[b], ph ^ 1);
-      tc::fence_after_sync();
-      const uint32_t td = tmem_base + ((uint32_t)(q * 32) << 16) + b * kMlpH + part * 48;
-      uint8_t* hr = s_h + b * kMlpHBytes + row * 16;
-      uint32_t va[16], vb[16], vc[16];
-      tc::tmem_ld16(td, va); tc::tmem_ld16(td + 16, vb); tc::tmem_ld16(td + 32, vc);
-      auto emit = [&](const uint32_t (&v)[16], int c16) {
+        for (int c = 0; c < kMlpC; ++c) sum += f[c];
+        const float mean = sum * (1.f / kMlpC);
+        float var = 0.f;
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int col = part * 48 + c16 * 16 + hh * 8;
-          float f[8];
+        for (int c = 0; c < kMlpC; ++c) { const float d = f[c] - mean; var = fmaf(d, d, var); }
+        const float rstd = 1.f / sqrtf(var * (1.f / kMlpC) + p.eps);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[hh * 8 + j]) + s_b1[col + j];
+        for (int c = 0; c < kMlpC / 8; ++c) {
           uint4 o;
           __half2* oh = reinterpret_cast<__half2*>(&o);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(gelu_erf(f[2 * j]), gelu_erf(f[2 * j + 1]));
-          *reinterpret_cast<uint4*>(hr + (col / 8) * 2048) = o;
+          for (int j = 0; j < 4; ++j) {
+            const int k = c * 8 + 2 * j;
+            oh[j] = __floats2half2_rn((f[k] - mean) * rstd * s_gamma[k] + s_beta[k], (f[k + 1] - mean) * rstd * s_gamma[k + 1] + s_beta[k + 1]);
+          }
+          *reinterpret_cast<uint4*>(xr + c * 2048) = o;
         }
-      };
-      tc::tmem_ld_wait16(va); emit(va, 0);
-      tc::tmem_ld_wait16(vb); emit(vb, 1);
-      tc::tmem_ld_wait16(vc); emit(vc, 2);
-      tc::fence_proxy_async();
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) { tc::mbar_arrive(&h_full[b]); tc::mbar_arrive(&d1_free[b]); }
+        tc::fence_proxy_async();   // generic-proxy stores -> visible to the wgmma operand reads
+      }
+      tc::wg_bar(8 + g);
+      // ---- GEMM1: D1 = LN(X) * W1^T (64 x 192) ----
+      float d1[kMlpH / 2];
+      tc::wg_fence();
+#pragma unroll
+      for (int k = 0; k < kMlpC / 16; ++k) {
+        const uint64_t ad = tc::make_desc_kmajor_noswz(x_a + b * kMlpXBytes + k * 4096 + g * 1024, 2048, 128);
+        const uint64_t bd = tc::make_desc_kmajor_noswz(w1_a + k * kMlpH * 32, kMlpH * 16, 128);
+        tc::wg_mma_ss<kMlpH>(d1, ad, bd, k != 0 ? 1u : 0u, 128);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc<kMlpH / 2>(d1);
+      if (wid == 0 && lane == 0) tc::mbar_arrive(&x_free[b]);
+      // ---- + b1, GELU, fp16: the D1 fragment of columns 16k .. 16k+15 is the A fragment of K-step k of GEMM2 ----
+      uint32_t a[kMlpH / 16][4];
+#pragma unroll
+      for (int k = 0; k < kMlpH / 16; ++k)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int col = 16 * k + 8 * (j >> 1) + c_lane;
+          const float* dv = d1 + 8 * k + 2 * j;
+          a[k][j] = pack_half2(gelu_erf(dv[0] + s_b1[col]), gelu_erf(dv[1] + s_b1[col + 1]));
+        }
+      // ---- GEMM2: D2 = H * W2^T (64 x 48) ----
+      float d2[kMlpC / 2];
+      tc::wg_fence();
+#pragma unroll
+      for (int k = 0; k < kMlpH / 16; ++k) {
+        const uint64_t bd = tc::make_desc_kmajor_noswz(w2_a + k * kMlpC * 32, kMlpC * 16, 128);
+        tc::Mma<kMlpC>::rs<0>(d2, a[k], bd, k != 0 ? 1u : 0u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc<kMlpC / 2>(d2);
+#pragma unroll
+      for (int k = 0; k < kMlpH / 16; ++k)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(a[k][j])::"memory");   // A registers stay live until the wait
+      // ---- epilogue: + b2 + x (the raw row, re-read from global memory: an L2 hit), NC8 store ----
+      const int r = rt * 128 + 64 * g + 32 * (wid & 1) + lane;
+      const bool ok = r < p.S;
+#pragma unroll
+      for (int c16 = 0; c16 < kMlpC / 16; ++c16, ++sl) {
+        float* buf = stage + (sl & 1) * tc::kStageFloats;
+        tc::wg_stage16<0>(d2 + c16 * 8, buf, wid, lane);
+        tc::wg_bar(8 + g);
+        float v[8];
+        tc::wg_read8(buf, wid, lane, v);
+        const int c = 2 * c16 + (wid >> 1);
+        if (ok) {
+          const uint4 res = __ldg(reinterpret_cast<const uint4*>(p.x + ((long long)n * (p.x_ctot / 8) * p.S + r) * 8 + (long long)c * p.S * 8));
+          const __half2* rh = reinterpret_cast<const __half2*>(&res);
+          uint4 o;
+          __half2* oh = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float2 rr = __half22float2(rh[j]);
+            const int k = c * 8 + 2 * j;
+            oh[j] = __floats2half2_rn(v[2 * j] + s_b2[k] + rr.x, v[2 * j + 1] + s_b2[k + 1] + rr.y);
+          }
+          *reinterpret_cast<uint4*>(p.y + ((long long)n * (p.y_ctot / 8) * p.S + r) * 8 + (long long)c * p.S * 8) = o;
+        }
+      }
     }
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, 512);
   }
 }
 

@@ -22,7 +22,7 @@ struct StatsPartials {
   float* buf;                 // [groups][R][rows_per_cta][2*NT]; null = no statistics
   int R;                      // min(tiles_per_group, gridDim.x)
   long long tiles_per_group;
-  int rows_per_cta;           // partial rows one CTA writes per group: 4 (one per TMEM lane quarter) x epilogue warp groups
+  int rows_per_cta;           // partial rows one CTA writes per group: 4 (one per 32-row quarter of the tile)
 };
 
 // flush the warp-private running sums of columns [col_lo, col_hi) (in {sum,sumsq} pairs) and clear them; `slot` = this

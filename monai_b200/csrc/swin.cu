@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(256) layernorm8_nc8_kernel(const __half* __res
 //   index(i, j) = lin(i) - lin(j) + const,  lin(t) = d*(2w1-1)(2w2-1) + h*(2w2-1) + w  with the token's coordinates in
 // the MODULE window (the reference slices relative_position_index[:n, :n], swin_unetr.py:514-516, so clamped windows
 // keep base-`window_size` coordinates).  With head_dim 16 the kernel is bound by exp/softmax issue, not by the MMAs,
-// which is why the legacy warp-level mma.sync path is used here instead of a tcgen05 + TMEM round trip (DESIGN.md 4.3).
+// which is why the legacy warp-level mma.sync path is used here instead of a tensor-memory round trip.
 constexpr int kAttKStride = 24;   // halfs per K row in smem (48 B: conflict-free b-fragment loads)
 
 __device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -660,7 +660,7 @@ extern "C" int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S,
   {
     // B200_HEAD_TC=1: tensor-core version (head_tc.cu) for the shapes it covers.  Off by default: both forms run at the same
     // 4.1-4.4 TB/s on the C3 head (44.1 ms against 42.0 ms per volume) -- twelve concurrent 2 KB streams per tile, not the FMAs, set
-    // the pace -- so the UMMA buys nothing here.
+    // the pace -- so a larger MMA buys nothing here.
     static const bool use_tc = std::getenv("B200_HEAD_TC") != nullptr;
     if (use_tc) {
       const int rc = launch_head_conv_norm_tc(x, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, slope, weight, bias, Cout, y,

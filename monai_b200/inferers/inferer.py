@@ -1,6 +1,6 @@
 """Inferer classes with the reference's constructor / call signatures (monai/inferers/inferer.py:62-97, 399-552).
 
-`SlidingWindowInferer` stores its arguments and calls the B200-native `sliding_window_inference` positionally,
+`SlidingWindowInferer` stores its arguments and calls the H100-native `sliding_window_inference` positionally,
 exactly as the reference does (inferer.py:532-552).  `SlidingWindowInfererAdapt` keeps its name and signature; the
 OOM ladder of the reference (inferer.py:565-641) degrades gracefully here because the resident-prediction budget
 already bounds memory, so it only adds the `cpu_thresh` bookkeeping.

@@ -1,4 +1,4 @@
-"""B200-native `sliding_window_inference` (drop-in for monai/inferers/utils.py:42-321).
+"""H100-native `sliding_window_inference` (drop-in for monai/inferers/utils.py:42-321).
 
 Same signature, argument meaning and error behaviour as the reference.  What differs is *how* the stitched
 volume is produced: windows are gathered by `b200_sw_gather`, and the importance-weighted overlap blend

@@ -1,11 +1,11 @@
-"""`SwinUNETR` (monai/networks/nets/swin_unetr.py:45-330, 919-1075) on tcgen05 tensor cores.
+"""`SwinUNETR` (monai/networks/nets/swin_unetr.py:45-330, 919-1075) on Hopper wgmma tensor cores.
 
 The module tree only holds parameters under the reference's names (159 state_dict keys for the default config:
 `swinViT.layers1.0.blocks.0.attn.qkv.weight`, `encoder1.layer.conv1.conv.weight`, `decoder5.transp_conv.conv.weight`,
 `out.conv.conv.bias`, ...), so reference checkpoints load unchanged.  `forward` never calls a torch op on activations:
 the whole network runs on fp16 channel-blocked ("NC8") buffers through the C ABI --
 
-  * 3x3x3 convolutions: implicit GEMM on tcgen05 (`b200_conv3x3x3_tc`), InstanceNorm partial sums in the epilogue;
+  * 3x3x3 convolutions: implicit GEMM on wgmma (`b200_conv3x3x3_tc`), InstanceNorm partial sums in the epilogue;
   * Linear / 1x1x1 conv / ConvTranspose k2 s2: `b200_gemm_tc` (bias, GELU, residual, window-reverse scatter,
     2x upsample scatter fused in the epilogue);
   * LayerNorm + pad + cyclic shift + window partition: one gather kernel (`b200_layernorm_nc8`);
@@ -372,7 +372,7 @@ class SwinUNETR(GraphedForward, nn.Module):
     def _plan(self, dims, ws, ss, dev):
         def build():
             src, region, nW, n = window_plan(dims, ws, ss)
-            # schedule of the tcgen05 attention: windows grouped by shift-mask pattern (at most 8 patterns)
+            # schedule of the tensor-core attention: windows grouped by shift-mask pattern (at most 8 patterns)
             sched, reps, ntypes = K.window_attention_tc_plan(region, nW, n)
             tc = None
             if ntypes <= 8 and n <= 352:
@@ -382,7 +382,7 @@ class SwinUNETR(GraphedForward, nn.Module):
         return self._cache.get(("plan", tuple(dims), tuple(ws), tuple(ss), dev), [], build)
 
     def _wqkv_scaled(self, attn: WindowAttention, key: str):
-        """qkv projection with scale * log2(e) folded into its q rows (the tcgen05 attention works in log2 units)."""
+        """qkv projection with scale * log2(e) folded into its q rows (the tensor-core attention works in log2 units)."""
         def build():
             C = attn.dim
             f = attn.scale * K.LOG2E
@@ -462,7 +462,7 @@ class SwinUNETR(GraphedForward, nn.Module):
             bkey = f"{key}.b{bi}"
             xw = K.layernorm_nc8(cur, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps, src=src, out_sp=(1, nW, n))
             if K.ATTN_TC and tc is not None:
-                # tcgen05 attention: bias + shift mask accumulated by the tensor core, scores in log2 units
+                # tensor-core attention: bias + shift mask accumulated by the tensor core, scores in log2 units
                 wq, bq = self._wqkv_scaled(blk.attn, bkey)
                 qkv, _ = K.gemm_tc(xw, wq, C, 3 * C, bias=bq)
                 att = K.window_attention_tc(qkv, C, blk.num_heads, nW, n, self._attn_bias(blk.attn, (bkey, tuple(dims), tuple(ws), tuple(ss)), n, tc), tc[0], tc[2])

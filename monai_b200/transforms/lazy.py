@@ -4,7 +4,7 @@ Restates monai/transforms/lazy/functional.py:195-296 (`apply_pending`), monai/tr
 composition, `resample`) and the pending-operation bookkeeping of monai/transforms/inverse.py:168-290.  A lazy transform does not
 touch the voxels: it pushes {lazy_affine: output voxel index -> input voxel index, lazy_shape, ...} onto
 `MetaTensor.pending_operations`; `apply_pending` multiplies the matrices in application order and hands the product to ONE
-`SpatialResample` launch (dst_affine = affine @ cumulative) -- on the B200 path one `b200_resample_affine` kernel whose
+`SpatialResample` launch (dst_affine = affine @ cumulative) -- on the GPU one `b200_resample_affine` kernel whose
 coordinates come from the composed matrix, so `Spacingd -> RandAffined` costs one pass over the volume instead of two.
 
 As in the reference, the interpolation / padding mode of the single resample comes from the pending items' top-level

@@ -1,7 +1,7 @@
 """Deterministic, name-keyed weights shared by make_golden.py (reference side) and the tests (monai_b200 side).
 
 Filling a state_dict through this function makes the weights independent of module construction order and RNG
-consumption, so the reference model and the B200 model are guaranteed to hold identical parameters.
+consumption, so the reference model and the H100 model are guaranteed to hold identical parameters.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""GPU parity of the general tcgen05 convolution (cp.async im2col producer): stride-1/2 Conv3d and ConvTranspose3d
+"""GPU parity of the general wgmma convolution (cp.async im2col producer): stride-1/2 Conv3d and ConvTranspose3d
 vs torch fp32 references on fp16-rounded operands (tolerance 2e-3 of the output scale, fp32 accumulation)."""
 import pytest
 import torch

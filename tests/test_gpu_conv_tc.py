@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM 3x3x3 convolution against a torch fp32 reference of the same op.
+"""GPU parity of the wgmma implicit-GEMM 3x3x3 convolution against a torch fp32 reference of the same op.
 
 Inputs and weights are rounded to fp16 first (the kernel's storage type), so the only differences left are the
 fp32 accumulation order and the final fp16 rounding of the output: tolerance 2e-3 relative to the output scale.

@@ -1,4 +1,4 @@
-"""GPU parity of the SwinUNETR path (tcgen05 convs / GEMMs, window attention, LayerNorm / merging kernels) against the
+"""GPU parity of the SwinUNETR path (wgmma convs / GEMMs, window attention, LayerNorm / merging kernels) against the
 reference fixtures (real MONAI outputs) and the torch-CPU oracle.  The network computes in fp16 with fp32
 accumulation, the oracle in fp32: tolerances are stated relative to the output scale."""
 import contextlib
@@ -154,7 +154,7 @@ def test_window_attention_matches_reference_math(ws, n, nW, heads):
 
 @pytest.mark.parametrize("ws,n,nW,heads", [((7, 7, 7), 343, 5, 3), ((7, 7, 7), 216, 3, 6), ((7, 7, 7), 8, 4, 24), ((7, 7, 7), 196, 9, 12)])
 def test_window_attention_tcgen05_matches_reference_math(ws, n, nW, heads):
-    """b200_window_attention_tc: bias + shift mask added by the tensor core, softmax from TMEM, P V on tcgen05."""
+    """b200_window_attention_tc: bias + shift mask added by the tensor core, online softmax in registers, P V on wgmma."""
     from monai_b200.networks.nets.swin_unetr import WindowAttention
 
     g = torch.Generator().manual_seed(5)
@@ -223,7 +223,7 @@ def test_instance_norm_statistics_are_deterministic():
 def test_cin1_stem_and_head(force_cuda_core):
     g = torch.Generator().manual_seed(4)
     x = torch.randn((2, 1, 8, 10, 12), generator=g)
-    K._FORCE_CUDA_CORE_STEM = force_cuda_core   # False: tcgen05 stems for (3,1,1) and (2,2,0); True: CUDA-core kernel for all
+    K._FORCE_CUDA_CORE_STEM = force_cuda_core   # False: wgmma stems for (3,1,1) and (2,2,0); True: CUDA-core kernel for all
     try:
         for k, s, p in [(3, 1, 1), (2, 2, 0), (1, 1, 0)]:
             w, b = torch.randn((48, 1, k, k, k), generator=g) / k**1.5, torch.randn(48, generator=g)
@@ -275,7 +275,7 @@ def test_fused_residual_tail_kernels():
 
 
 def test_head_on_tensor_cores_many_tiles_and_classes():
-    """head_conv_norm_nc8 at C = 48 (with B200_HEAD_TC=1: one UMMA per 128 voxels, head_tc.cu): 14 classes, several batch items, a
+    """head_conv_norm_nc8 at C = 48 (with B200_HEAD_TC=1: wgmma per 128 voxels, head_tc.cu): 14 classes, several batch items, a
     ragged last tile, fp16 and fp32 logits -- against torch fp32 (dynunet_block.py:104-111 + 247-267)."""
     g = torch.Generator().manual_seed(5)
     N, C, sp, CO = 3, 48, (9, 20, 23), 14
@@ -296,7 +296,7 @@ def test_head_on_tensor_cores_many_tiles_and_classes():
 
 
 def test_head_tensor_core_variant_in_a_subprocess():
-    """The opt-in UMMA form of the head (B200_HEAD_TC=1, read once per process) against the same references."""
+    """The opt-in wgmma form of the head (B200_HEAD_TC=1, read once per process) against the same references."""
     import subprocess
     import sys
 

@@ -76,7 +76,7 @@ def test_basic_unet_matches_reference_fixture(golden_dir):
 
 
 def test_unet_tensor_core_path_matches_direct_path(monkeypatch):
-    """fp16 UNet (C2 topology): tcgen05 im2col path (NC8, CUDA-graph replay) vs the CUDA-core NCDHW path."""
+    """fp16 UNet (C2 topology): wgmma im2col path (NC8, CUDA-graph replay) vs the CUDA-core NCDHW path."""
     net = _build(lambda: UNet(3, 1, 2, (16, 32, 64, 128, 256), (2, 2, 2, 2)), 1).half()
     x = torch.randn(3, 1, 32, 48, 64, generator=torch.Generator().manual_seed(5)).to(DEV).half()
     assert net._tc_eligible(x)
