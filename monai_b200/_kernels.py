@@ -665,13 +665,11 @@ def gemm_tc(
     return out, stats
 
 
-RES_FOLD = os.environ.get("B200_RES_UNFOLDED", "") == ""   # B200_RES_UNFOLDED=1: the 1x1x1 residual convolution as its own gemm_tc launch
-NORM_ON_LOAD = os.environ.get("B200_NORM_UNFUSED", "") == ""   # B200_NORM_UNFUSED=1: norm_act_nc8 pass between conv1 and conv2 (A/B measurements)
-MLP_FUSED = os.environ.get("B200_MLP_UNFUSED", "") == ""   # B200_MLP_UNFUSED=1: layernorm_nc8 + two gemm_tc (A/B measurements)
+NORM_ON_LOAD = os.environ.get("B200_NORM_UNFUSED", "") == ""   # B200_NORM_UNFUSED=1: norm_act_nc8 pass between conv1 and conv2 (DESIGN.md §9)
 
 
 def mlp_fused_supported(C_: int, hidden: int) -> bool:
-    return MLP_FUSED and C_ == 48 and hidden == 192
+    return C_ == 48 and hidden == 192
 
 
 def mlp_fused_tc(x: NC8, packed_w1: torch.Tensor, b1: torch.Tensor, packed_w2: torch.Tensor, b2: torch.Tensor, hidden: int,
@@ -712,9 +710,6 @@ def window_attention_nc8(qkv: NC8, Cc: int, heads: int, nW: int, n: int, scale: 
           L.ptr(region), L.ptr(out.buf), L.stream_ptr(qkv.buf.device), flops=4.0 * qkv.N * nW * heads * n * n * 16,
           nbytes=float(qkv.N * 4 * Cc * nW * n * 2))
     return out
-
-
-_FORCE_CUDA_CORE_STEM = bool(os.environ.get("B200_STEM_CUDA_CORE"))
 
 
 def window_attention_tc_plan(region, nW: int, n: int):
@@ -772,7 +767,7 @@ def window_attention_tc(qkv: NC8, Cc: int, heads: int, nW: int, n: int, packed_b
     return out
 
 
-ATTN_TC = not bool(os.environ.get("B200_ATTN_HMMA"))   # tensor-core attention unless the mma.sync kernel is forced (debugging)
+ATTN_TC = not bool(os.environ.get("B200_ATTN_HMMA"))   # B200_ATTN_HMMA=1: mma.sync window_attention_nc8 for every window (DESIGN.md §9)
 LOG2E = 1.4426950408889634
 
 
@@ -790,7 +785,7 @@ def conv_cin1_nc8(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | No
     b32 = _f32c(bias)
     stats = torch.empty((N * Cout, 2), device=x.device, dtype=torch.float32) if want_stats else None
     # tensor-core stem for the shapes it covers (the 3x3x3 stem and the patch embedding); CUDA-core kernel otherwise
-    tc = (k, stride, pad) in ((3, 1, 1), (2, 2, 0)) and Cout in (16, 32, 48, 64, 96, 128) and not _FORCE_CUDA_CORE_STEM
+    tc = (k, stride, pad) in ((3, 1, 1), (2, 2, 0)) and Cout in (16, 32, 48, 64, 96, 128)
     name = "conv_cin1_tc" if tc else "conv_cin1_nc8"
     ws = None
     if want_stats:

@@ -9,9 +9,7 @@
 // never materialised.  imp() is evaluated on the fly from the three 1-D
 // vectors of compute_importance_map (monai/data/utils.py:1084-1134): ((g_d*g_h)*g_w) clamped from below.
 #include "common.cuh"
-#include "tc90.cuh"
 #include "blend.cuh"
-#include <cstdlib>
 #include "../../include/monai_b200.h"
 
 namespace b200 {
@@ -401,161 +399,6 @@ __global__ void __launch_bounds__(32 * kBlend8Rows, sizeof(TP) == 2 ? 2 : 1) sw_
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// TMA-staged blend (fp16 predictions, modes 0 / 1).  A block owns an output tile of kTmaTH rows x kTmaTW voxels of one
-// depth plane and walks, in ascending window index, every window that intersects the tile.  A producer warp fetches the
-// tile's footprint inside each window with ONE 5-D TMA box load (box = TW x TH x 1 x C x 1 of the prediction store
-// [win][C][rd][rh][rw]; coordinates outside the window are zero-filled by the TMA unit, negative ones included) into a
-// ring of shared-memory stages, so address arithmetic and memory-level parallelism cost no SM instructions; four consumer
-// warps (four voxels per thread) evaluate the importance weight analytically, accumulate with one FMA per term and
-// divide at the end.  A window that does not cover a voxel contributes an exact zero to its numerator and to its weight
-// sum, so the result is bit-identical to sw_blend8_kernel / sw_blend_kernel on fp16 predictions.
-// ---------------------------------------------------------------------------------------------------------------
-constexpr int kTmaTH = 8, kTmaTW = 64, kTmaStages = 8, kTmaMaxC = 8, kTmaMaxRoi = 512;
-
-struct BlendTmaParams {
-  BlendParams b;
-  int stage_bytes;   // C * TH * TW * 2
-};
-
-template <typename TO, int MODE, int CMAX>
-__global__ void __launch_bounds__(160) sw_blend_tma_kernel(const __grid_constant__ CUtensorMap tmap, BlendTmaParams q) {
-  extern __shared__ uint8_t s_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(s_raw) + 127) & ~uintptr_t(127));
-  const BlendParams& p = q.b;
-  uint8_t* stages = smem;
-  uint64_t* full = reinterpret_cast<uint64_t*>(stages + kTmaStages * q.stage_bytes);
-  uint64_t* empty = full + kTmaStages;
-  float* s_gh = reinterpret_cast<float*>(empty + kTmaStages);   // [rh]
-  float* s_gw = s_gh + p.rh;                                     // [rw]
-  __shared__ int s_rng[6];                                       // window index ranges [lo, hi) per axis for this tile
-
-  const int nd_box = p.d1 - p.d0;
-  const int d = blockIdx.z % nd_box + p.d0, b = blockIdx.z / nd_box;
-  const int h0 = p.h0 + blockIdx.y * kTmaTH, w0 = blockIdx.x * kTmaTW;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kTmaStages; ++i) { tc::mbar_init(&full[i], 1); tc::mbar_init(&empty[i], 128); }
-    tc::fence_barrier_init();
-  }
-  if (threadIdx.x < 3) {
-    // sorted starts: the windows that intersect [x0, x1) along an axis form a contiguous index range
-    const int ax = threadIdx.x;
-    const int* st = ax == 0 ? p.starts_d : (ax == 1 ? p.starts_h : p.starts_w);
-    const int ns = ax == 0 ? p.nd : (ax == 1 ? p.nh : p.nw), r = ax == 0 ? p.rd : (ax == 1 ? p.rh : p.rw);
-    const int x0 = ax == 0 ? d : (ax == 1 ? h0 : w0), x1 = ax == 0 ? d + 1 : (ax == 1 ? min(h0 + kTmaTH, p.h1) : min(w0 + kTmaTW, p.W));
-    int lo = ns, hi = 0;
-    for (int i = 0; i < ns; ++i) { const int s = __ldg(st + i); if (s < x1 && s + r > x0) { lo = min(lo, i); hi = max(hi, i + 1); } }
-    s_rng[2 * ax] = lo; s_rng[2 * ax + 1] = max(hi, lo);
-  }
-  for (int i = threadIdx.x; i < p.rh; i += blockDim.x) s_gh[i] = __ldg(p.gh + i);
-  for (int i = threadIdx.x; i < p.rw; i += blockDim.x) s_gw[i] = __ldg(p.gw + i);
-  __syncthreads();
-  const int id_lo = s_rng[0], id_hi = s_rng[1], ih_lo = s_rng[2], ih_hi = s_rng[3], iw_lo = s_rng[4], iw_hi = s_rng[5];
-  const int num_win = p.nd * p.nh * p.nw;
-
-  if (warp == 4) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      tc::tma_prefetch_desc(&tmap);
-      int s = 0; uint32_t ph = 0;
-      for (int id = id_lo; id < id_hi; ++id) {
-        const int sd = __ldg(p.starts_d + id);
-        for (int ih = ih_lo; ih < ih_hi; ++ih) {
-          const int sh = __ldg(p.starts_h + ih);
-          for (int iw = iw_lo; iw < iw_hi; ++iw) {
-            const int widx = b * num_win + (id * p.nh + ih) * p.nw + iw;
-            if (widx < p.win_begin || widx >= p.win_end) continue;
-            const int sw = __ldg(p.starts_w + iw);
-            tc::mbar_wait(&empty[s], ph ^ 1);
-            tc::mbar_arrive_expect_tx(&full[s], q.stage_bytes);
-            tc::tma_load_5d(stages + s * q.stage_bytes, &tmap, &full[s], w0 - sw, h0 - sh, d - sd, 0, widx - p.win_begin);
-            if (++s == kTmaStages) { s = 0; ph ^= 1; }
-          }
-        }
-      }
-    }
-    return;
-  }
-  // ===================== consumers: thread = (row, four consecutive voxels) =====================
-  const int row = threadIdx.x >> 4, cg = threadIdx.x & 15;
-  const int h = h0 + row, w = w0 + cg * 4;
-  const long long vol = (long long)p.D * p.H * p.W;
-  const long long voff = ((long long)d * p.H + h) * p.W + w;
-  const bool in_vol = h < p.h1 && w < p.W;   // W % 4 == 0: the four voxels are inside together
-  float cnt[4] = {0.f, 0.f, 0.f, 0.f};
-  float acc[CMAX][4];
-#pragma unroll
-  for (int c = 0; c < CMAX; ++c) {
-    acc[c][0] = acc[c][1] = acc[c][2] = acc[c][3] = 0.f;
-    if (MODE == 1 && c < p.C && in_vol) {
-      const float4 a = *reinterpret_cast<const float4*>((const float*)p.out + ((long long)b * p.C + c) * vol + voff);
-      acc[c][0] = a.x; acc[c][1] = a.y; acc[c][2] = a.z; acc[c][3] = a.w;
-    }
-  }
-  int s = 0; uint32_t ph = 0;
-  for (int id = id_lo; id < id_hi; ++id) {
-    const int ld = d - __ldg(p.starts_d + id);
-    const float gdv = __ldg(p.gd + ld);
-    for (int ih = ih_lo; ih < ih_hi; ++ih) {
-      const int lh = h - __ldg(p.starts_h + ih);
-      const bool hcov = lh >= 0 && lh < p.rh;
-      const float gdh = __fmul_rn(gdv, s_gh[hcov ? lh : 0]);
-      for (int iw = iw_lo; iw < iw_hi; ++iw) {
-        const int widx = b * num_win + (id * p.nh + ih) * p.nw + iw;
-        const bool res = widx >= p.win_begin && widx < p.win_end;
-        const int lw = w - __ldg(p.starts_w + iw);
-        // weights of this window at the thread's four voxels (0 where the window does not cover the voxel)
-        float t[4];
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          const int l = lw + v;
-          const bool cov = hcov && l >= 0 && l < p.rw;
-          t[v] = cov ? fmaxf(__fmul_rn(gdh, s_gw[cov ? l : 0]), p.clamp_min) : 0.f;
-          cnt[v] = __fadd_rn(cnt[v], t[v]);
-        }
-        if (!res) continue;                     // only resident windows were fetched (mode 0 is called with all of them resident)
-        tc::mbar_wait(&full[s], ph);
-        const uint8_t* st = stages + s * q.stage_bytes + (row * kTmaTW + cg * 4) * 2;
-#pragma unroll
-        for (int c = 0; c < CMAX; ++c) {
-          if (c < p.C) {
-            const uint2 raw = *reinterpret_cast<const uint2*>(st + c * (kTmaTH * kTmaTW * 2));
-            const float2 x01 = __half22float2(*reinterpret_cast<const __half2*>(&raw.x));
-            const float2 x23 = __half22float2(*reinterpret_cast<const __half2*>(&raw.y));
-            acc[c][0] = fmaf(x01.x, t[0], acc[c][0]); acc[c][1] = fmaf(x01.y, t[1], acc[c][1]);
-            acc[c][2] = fmaf(x23.x, t[2], acc[c][2]); acc[c][3] = fmaf(x23.y, t[3], acc[c][3]);
-          }
-        }
-        tc::mbar_arrive(&empty[s]);
-        if (++s == kTmaStages) { s = 0; ph ^= 1; }
-      }
-    }
-  }
-  if (!in_vol) return;
-#pragma unroll
-  for (int c = 0; c < CMAX; ++c) {
-    if (c < p.C) {
-      const long long o = ((long long)b * p.C + c) * vol + voff;
-      if (MODE == 0) {
-        float r[4];
-#pragma unroll
-        for (int v = 0; v < 4; ++v) r[v] = BlendFin<TO>::apply(acc[c][v], BlendFin<TO>::prep(cnt[v]));
-        if (sizeof(TO) == 2) {
-          uint2 o2;
-          *reinterpret_cast<__half2*>(&o2.x) = __floats2half2_rn(r[0], r[1]);
-          *reinterpret_cast<__half2*>(&o2.y) = __floats2half2_rn(r[2], r[3]);
-          *reinterpret_cast<uint2*>((__half*)p.out + o) = o2;
-        } else {
-          *reinterpret_cast<float4*>((float*)p.out + o) = make_float4(r[0], r[1], r[2], r[3]);
-        }
-      } else {
-        *reinterpret_cast<float4*>((float*)p.out + o) = make_float4(acc[c][0], acc[c][1], acc[c][2], acc[c][3]);
-      }
-    }
-  }
-}
-
 template <typename TI, typename TO>
 __global__ void __launch_bounds__(256) sw_gather_kernel(const TI* __restrict__ vol, TO* __restrict__ out,
                                                         const int* __restrict__ tab, int C, int D, int H, int W,
@@ -623,35 +466,6 @@ static int launch_blend_v(const BlendParams& p, int pred_dtype, int out_dtype, c
   }
 #undef LB
   B200_LAUNCH_CHECK("sw_blend_kernel");
-  return B200_OK;
-}
-
-template <int MODE>
-static int launch_blend_tma(const BlendParams& p, int out_dtype, cudaStream_t st) {
-  EncodeTiledFn enc = get_encode_tiled();
-  B200_REQUIRE(enc != nullptr, "sw_blend: cuTensorMapEncodeTiled entry point unavailable");
-  const int nres = p.win_end - p.win_begin;
-  CUtensorMap tmap;
-  cuuint64_t gdim[5] = {(cuuint64_t)p.rw, (cuuint64_t)p.rh, (cuuint64_t)p.rd, (cuuint64_t)p.C, (cuuint64_t)nres};
-  cuuint64_t gstr[4] = {(cuuint64_t)p.ps_h * 2, (cuuint64_t)p.ps_d * 2, (cuuint64_t)p.ps_c * 2, (cuuint64_t)p.ps_n * 2};
-  cuuint32_t box[5] = {(cuuint32_t)kTmaTW, (cuuint32_t)kTmaTH, 1, (cuuint32_t)p.C, 1};
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(p.preds), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  B200_REQUIRE(r == CUDA_SUCCESS, "sw_blend: cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
-  BlendTmaParams q;
-  q.b = p; q.stage_bytes = p.C * kTmaTH * kTmaTW * 2;
-  dim3 grid(ceil_div(p.W, kTmaTW), ceil_div(p.h1 - p.h0, kTmaTH), (p.d1 - p.d0) * p.B);
-  if (grid.y == 0 || grid.z == 0) return B200_OK;
-  B200_REQUIRE(grid.z <= 65535 && grid.y <= 65535, "sw_blend: volume too large for the launch grid");
-  const size_t smem = (size_t)kTmaStages * q.stage_bytes + 2 * kTmaStages * 8 + (size_t)(p.rh + p.rw) * 4 + 256;
-#define LT(TO, CM) do { B200_CUDA(cudaFuncSetAttribute(sw_blend_tma_kernel<TO, MODE, CM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); \
-                        sw_blend_tma_kernel<TO, MODE, CM><<<grid, 160, smem, st>>>(tmap, q); } while (0)
-#define LTC(TO) do { if (p.C <= 2) LT(TO, 2); else if (p.C <= 4) LT(TO, 4); else LT(TO, 8); } while (0)
-  if (MODE == 1 || out_dtype == B200_DT_F32) LTC(float); else LTC(__half);
-#undef LTC
-#undef LT
-  B200_LAUNCH_CHECK("sw_blend_tma_kernel");
   return B200_OK;
 }
 
@@ -727,20 +541,9 @@ extern "C" int b200_sw_blend(const b200_blend_desc* dsc, int mode, void* stream)
     vec8 = (reinterpret_cast<uintptr_t>(p.preds) % 16 == 0) && p.ps_n % 8 == 0 && p.ps_c % 8 == 0 && p.ps_d % 8 == 0 && p.ps_h % 8 == 0;
   if (p.slot_map) vec8 = false;   // only the general kernel looks windows up through a slot map
   // lean 8-voxel kernel: everything resident, fp16 predictions, separable weights, at most three covering windows per axis
-  static int no_lean = -1;
-  if (no_lean < 0) { const char* e = getenv("B200_BLEND_NO_LEAN"); no_lean = (e && e[0] == '1') ? 1 : 0; }
-  if (!no_lean && mode == 0 && vec8 && dsc->pred_dtype == B200_DT_F16 && !p.wmap && dsc->max_cover >= 1 && dsc->max_cover <= 3 && p.rw <= 512 &&
+  if (mode == 0 && vec8 && dsc->pred_dtype == B200_DT_F16 && !p.wmap && dsc->max_cover >= 1 && dsc->max_cover <= 3 && p.rw <= 512 &&
       p.win_begin == 0 && p.win_end == p.B * p.nd * p.nh * p.nw)
     return launch_blend8_lean(p, dsc->out_dtype, st);
-  // TMA-staged kernel: fp16 predictions, contiguous window rows, 16-byte aligned strides, separable importance factors
-  static int use_tma = -1;
-  if (use_tma < 0) { const char* e = getenv("B200_BLEND_TMA"); use_tma = (e && e[0] == '1') ? 1 : 0; }   // opt-in until validated on the GPU
-  const bool tma_ok = use_tma && !p.slot_map && mode != 2 && dsc->pred_dtype == B200_DT_F16 && !p.wmap && p.ps_w == 1 && p.C <= kTmaMaxC && p.W % 4 == 0 &&
-                      p.rw % 8 == 0 && p.rh <= kTmaMaxRoi && p.rw <= kTmaMaxRoi && p.rh >= kTmaTH && p.rw >= kTmaTW && p.ps_h % 8 == 0 && p.ps_d % 8 == 0 && p.ps_c % 8 == 0 &&
-                      p.ps_n % 8 == 0 && reinterpret_cast<uintptr_t>(p.preds) % 16 == 0 && reinterpret_cast<uintptr_t>(p.out) % 16 == 0 &&
-                      p.win_end > p.win_begin && (long long)p.ps_h * 2 < (1LL << 40);
-  if (tma_ok && mode == 0) return launch_blend_tma<0>(p, dsc->out_dtype, st);
-  if (tma_ok && mode == 1) return launch_blend_tma<1>(p, dsc->out_dtype, st);
   if (mode == 0) return launch_blend<0>(p, dsc->pred_dtype, dsc->out_dtype, vec2, vec8, st);
   if (mode == 1) return launch_blend<1>(p, dsc->pred_dtype, dsc->out_dtype, vec2, vec8, st);
   return launch_blend<2>(p, dsc->pred_dtype, dsc->out_dtype, vec2, vec8, st);

@@ -7,7 +7,6 @@
 // Sampling semantics follow ATen grid_sampler_3d (unnormalised coordinates are produced by the host):
 //   padding zeros / border / reflection (reflection bounds depend on align_corners), nearest = round-half-even.
 #include "common.cuh"
-#include <cstdlib>
 #include "../../include/monai_b200.h"
 
 namespace b200 {
@@ -159,139 +158,6 @@ __global__ void __launch_bounds__(256) resample_affine_kernel(ResampleP p) {
   }
 }
 
-// Shared-memory tiled form of the trilinear / zeros (MODE 0) and border (MODE 3) paths -- an EXPERIMENT that did not pay off (see
-// the dispatcher); kept opt-in because it is bit-identical and documents the result.
-//
-// The gather kernel above issues eight scalar global loads per output voxel (130 instructions per voxel, 0.10 of the HBM
-// bandwidth on the C4 shapes).  Here a block owns an 8 (d) x 8 (h) x 32 (w) OUTPUT tile: the source coordinates of a tile are an
-// affine image of a box, so their bounding box (from the eight tile corners, in fp64, clamped into the volume, + the far
-// interpolation corner) is a small source box -- 9 x 9 x 28 elements for Spacing 1.25 -> 1 mm, 18 x 18 x 37 for the rotated /
-// scaled RandAffine of C4 -- which the block copies once with coalesced row reads and then interpolates from shared memory.
-// Per-voxel arithmetic (fp64 base coordinate per 4-voxel group, fp32 increments, corner clamping, weight products, the order of
-// the eight FMAs) is the code of resample_affine_kernel, only the operand comes from the staged copy: results are bit-identical.
-// A tile whose source box does not fit (strong down-sampling) reads global memory like the gather kernel.
-constexpr int kRtD = 8, kRtH = 8, kRtW = 32;
-constexpr int kRtSmemFloats = 12 * 1024 - 16; // just under the 48 KB static limit: source box per channel pass
-
-template <typename TI, typename TO, int MODE>
-__global__ void __launch_bounds__(256) resample_affine_tiled_kernel(ResampleP p) {
-  static_assert(MODE == 0 || MODE == 3, "tiled path: trilinear with zeros or border padding");
-  __shared__ float s_box[kRtSmemFloats];
-  __shared__ int s_lo[3], s_n[3];
-  const int k_t = blockIdx.x * kRtW, j_t = blockIdx.y * kRtH, i_t = blockIdx.z * kRtD;
-  if (threadIdx.x == 0) {
-    // bounding box of the tile's source coordinates: extremes of an affine map over a box are attained at its corners
-    double lo[3] = {1e300, 1e300, 1e300}, hi[3] = {-1e300, -1e300, -1e300};
-    const int ie = min(i_t + kRtD, p.Do) - 1, je = min(j_t + kRtH, p.Ho) - 1, ke = min(k_t + kRtW, p.Wo) - 1;
-    for (int c = 0; c < 8; ++c) {
-      const double i = (c & 4) ? ie : i_t, j = (c & 2) ? je : j_t, k = (c & 1) ? ke : k_t;
-      for (int a = 0; a < 3; ++a) {
-        const double v = fma(p.m[4 * a], i, fma(p.m[4 * a + 1], j, fma(p.m[4 * a + 2], k, p.m[4 * a + 3])));
-        lo[a] = fmin(lo[a], v); hi[a] = fmax(hi[a], v);
-      }
-    }
-    const int size[3] = {p.Di, p.Hi, p.Wi};
-    for (int a = 0; a < 3; ++a) {
-      // one element of slack on both sides covers the fp32 increments (< 1e-6 voxel); + 1 for the far corner
-      const double l = fmin(1.0e9, fmax(-1.0e9, lo[a])), h = fmin(1.0e9, fmax(-1.0e9, hi[a]));
-      const int l_i = min(max((int)floor(l) - 1, 0), size[a] - 1), h_i = min(max((int)floor(h) + 2, 0), size[a] - 1);
-      s_lo[a] = l_i; s_n[a] = h_i - l_i + 1;
-    }
-  }
-  __syncthreads();
-  const int la = s_lo[0], lb = s_lo[1], lc = s_lo[2], na = s_n[0], nb = s_n[1], nc = s_n[2];
-  const long long nbox = (long long)na * nb * nc;
-  const bool staged = nbox <= kRtSmemFloats;
-  const long long in_cs = (long long)p.Di * p.Hi * p.Wi, out_cs = (long long)p.Do * p.Ho * p.Wo;
-  const TI* src = (const TI*)p.src;
-  TO* dst = (TO*)p.dst;
-  // thread -> two groups of four consecutive W voxels: (quad 0..7 along W, row 0..7 along H, planes dz and dz + 4)
-  const int tq = threadIdx.x & 7, tj = (threadIdx.x >> 3) & 7, tz = threadIdx.x >> 6;   // tz 0..3
-  const float sa = (float)p.m[2], sb = (float)p.m[6], sc = (float)p.m[10];
-  for (int ch = 0; ch < p.C; ++ch) {
-    const TI* s = src + ch * in_cs;
-    if (staged) {
-      if (ch > 0) __syncthreads();          // every thread has finished reading the previous channel's box
-      // a warp copies whole source rows (one division per row, lanes along W: coalesced); a per-element index decomposition cost more
-      // instructions than the interpolation itself
-      for (int r = threadIdx.x >> 5; r < na * nb; r += 8) {
-        const int a = r / nb, b = r - a * nb;
-        const TI* row = s + ((long long)(la + a) * p.Hi + (lb + b)) * p.Wi + lc;
-        float* drow = s_box + r * nc;
-        for (int c = threadIdx.x & 31; c < nc; c += 32) drow[c] = io<TI>::ld(row + c);
-      }
-      __syncthreads();
-    }
-#pragma unroll 1
-    for (int half = 0; half < 2; ++half) {
-      const int i = i_t + tz + 4 * half, j = j_t + tj, k0 = k_t + tq * kRsVox;
-      if (i >= p.Do || j >= p.Ho || k0 >= p.Wo) continue;
-      const double a = fma(p.m[0], (double)i, fma(p.m[1], (double)j, fma(p.m[2], (double)k0, p.m[3])));
-      const double b = fma(p.m[4], (double)i, fma(p.m[5], (double)j, fma(p.m[6], (double)k0, p.m[7])));
-      const double c = fma(p.m[8], (double)i, fma(p.m[9], (double)j, fma(p.m[10], (double)k0, p.m[11])));
-      const double lim = 1.0e9;
-      const double ac = fmin(lim, fmax(-lim, a)), bc = fmin(lim, fmax(-lim, b)), cc = fmin(lim, fmax(-lim, c));
-      const double fa0 = floor(ac), fb0 = floor(bc), fc0 = floor(cc);
-      const int IA = (int)fa0, IB = (int)fb0, IC = (int)fc0;
-      const float FA = (float)(ac - fa0), FB = (float)(bc - fb0), FC = (float)(cc - fc0);
-      float r[kRsVox];
-#pragma unroll
-      for (int v = 0; v < kRsVox; ++v) {
-        const float av = fmaf((float)v, sa, FA), bv = fmaf((float)v, sb, FB), cv = fmaf((float)v, sc, FC);
-        const float fa = floorf(av), fb = floorf(bv), fc = floorf(cv);
-        int a0 = IA + (int)fa, b0 = IB + (int)fb, c0 = IC + (int)fc;
-        float ta = av - fa, tb = bv - fb, tc = cv - fc;
-        if (MODE == 3) {
-          if (a0 < 0) { a0 = 0; ta = 0.f; } else if (a0 >= p.Di - 1) { a0 = p.Di - 1; ta = 0.f; }
-          if (b0 < 0) { b0 = 0; tb = 0.f; } else if (b0 >= p.Hi - 1) { b0 = p.Hi - 1; tb = 0.f; }
-          if (c0 < 0) { c0 = 0; tc = 0.f; } else if (c0 >= p.Wi - 1) { c0 = p.Wi - 1; tc = 0.f; }
-        }
-        float wa[2] = {1.f - ta, ta}, wb[2] = {1.f - tb, tb}, wc[2] = {1.f - tc, tc};
-        int a0c = a0, b0c = b0, c0c = c0, a1c, b1c, c1c;
-        if (MODE == 3) {
-          a1c = min(a0 + 1, p.Di - 1); b1c = min(b0 + 1, p.Hi - 1); c1c = min(c0 + 1, p.Wi - 1);
-        } else {
-          if (a0 < 0 || a0 >= p.Di) wa[0] = 0.f;
-          if (a0 + 1 < 0 || a0 + 1 >= p.Di) wa[1] = 0.f;
-          if (b0 < 0 || b0 >= p.Hi) wb[0] = 0.f;
-          if (b0 + 1 < 0 || b0 + 1 >= p.Hi) wb[1] = 0.f;
-          if (c0 < 0 || c0 >= p.Wi) wc[0] = 0.f;
-          if (c0 + 1 < 0 || c0 + 1 >= p.Wi) wc[1] = 0.f;
-          a0c = min(max(a0, 0), p.Di - 1); a1c = min(max(a0 + 1, 0), p.Di - 1);
-          b0c = min(max(b0, 0), p.Hi - 1); b1c = min(max(b0 + 1, 0), p.Hi - 1);
-          c0c = min(max(c0, 0), p.Wi - 1); c1c = min(max(c0 + 1, 0), p.Wi - 1);
-        }
-        // the clamped corners lie inside the staged box by construction; a defensive test keeps a surprise (NaN matrix) on the
-        // global path instead of reading outside shared memory
-        const bool in_box = staged && a0c >= la && a1c < la + na && b0c >= lb && b1c < lb + nb && c0c >= lc && c1c < lc + nc;
-        float acc = 0.f;
-        if (in_box) {
-          const int base = ((a0c - la) * nb + (b0c - lb)) * nc + (c0c - lc);
-          const int dD = (a1c - a0c) * nb * nc, dH = (b1c - b0c) * nc, dW = c1c - c0c;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const int da = q >> 2, db = (q >> 1) & 1, dc = q & 1;
-            acc = fmaf(s_box[base + (da ? dD : 0) + (db ? dH : 0) + (dc ? dW : 0)], wa[da] * wb[db] * wc[dc], acc);
-          }
-        } else {
-          const int base = (a0c * p.Hi + b0c) * p.Wi + c0c;
-          const int dD = (a1c - a0c) * p.Hi * p.Wi, dH = (b1c - b0c) * p.Wi, dW = c1c - c0c;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const int da = q >> 2, db = (q >> 1) & 1, dc = q & 1;
-            acc = fmaf(io<TI>::ld(s + base + (da ? dD : 0) + (db ? dH : 0) + (dc ? dW : 0)), wa[da] * wb[db] * wc[dc], acc);
-          }
-        }
-        r[v] = acc;
-      }
-      const long long o0 = ((long long)i * p.Ho + j) * p.Wo + k0;
-#pragma unroll
-      for (int v = 0; v < kRsVox; ++v)
-        if (k0 + v < p.Wo) io<TO>::st(dst + ch * out_cs + o0 + v, r[v]);
-    }
-  }
-}
-
 // out[i] = sum_t taps[t] * in[i + (t - r) * stride] along one axis, zero outside.
 template <typename TI, typename TO>
 __global__ void __launch_bounds__(256) filter1d_kernel(const TI* __restrict__ in, TO* __restrict__ out,
@@ -429,17 +295,8 @@ extern "C" int b200_resample_affine(const void* src, int src_dtype, int C, int D
   p.interp = interp; p.pad = pad; p.align = align_corners;
   dim3 block(32, 8), grid(ceil_div(Wo, 32 * kRsVox), ceil_div(Ho, 8), Do);
   cudaStream_t st = (cudaStream_t)stream;
-  // B200_RESAMPLE_TILED=1 selects the shared-memory tiled kernel for trilinear + zeros / border.  It is OFF by default: measured on
-  // the C4 shapes it is SLOWER than the gather kernel (Spacing 256^3 -> 320^3: 0.356 vs 0.246 ms; rotated 320^3: 0.66 vs 0.43 ms) --
-  // the gather's eight loads per voxel hit L1 / L2 (neighbouring voxels share corners), while the tile pays a block-wide copy, two
-  // barriers per channel and 48 KB of shared memory per block (4 blocks per SM) for the same DRAM traffic.
-  static const bool want_tiled = std::getenv("B200_RESAMPLE_TILED") != nullptr;
-  const bool tiled = want_tiled && interp == 1 && pad != 2 && ceil_div(Do, kRtD) <= 65535 && ceil_div(Ho, kRtH) <= 65535;
-  dim3 tgrid(ceil_div(Wo, kRtW), ceil_div(Ho, kRtH), ceil_div(Do, kRtD));
 #define LR(TI, TO) do { if (interp == 0) resample_affine_kernel<TI, TO, 2><<<grid, block, 0, st>>>(p); \
                        else if (pad == 2) resample_affine_kernel<TI, TO, 1><<<grid, block, 0, st>>>(p); \
-                       else if (tiled && pad == 1) resample_affine_tiled_kernel<TI, TO, 3><<<tgrid, 256, 0, st>>>(p); \
-                       else if (tiled) resample_affine_tiled_kernel<TI, TO, 0><<<tgrid, 256, 0, st>>>(p); \
                        else if (pad == 1) resample_affine_kernel<TI, TO, 3><<<grid, block, 0, st>>>(p); \
                        else resample_affine_kernel<TI, TO, 0><<<grid, block, 0, st>>>(p); } while (0)
   if (src_dtype == B200_DT_F32 && dst_dtype == B200_DT_F32) LR(float, float);

@@ -5,7 +5,6 @@
 // monai/networks/blocks/dynunet_block.py:247-267.
 #include "common.cuh"
 #include "stats.cuh"
-#include <cstdlib>
 #include "../../include/monai_b200.h"
 
 namespace b200 {
@@ -256,8 +255,9 @@ __global__ void __launch_bounds__(256) layernorm8_nc8_kernel(const __half* __res
 // The relative-position bias is looked up in the (2w-1)^3-entry table held in shared memory:
 //   index(i, j) = lin(i) - lin(j) + const,  lin(t) = d*(2w1-1)(2w2-1) + h*(2w2-1) + w  with the token's coordinates in
 // the MODULE window (the reference slices relative_position_index[:n, :n], swin_unetr.py:514-516, so clamped windows
-// keep base-`window_size` coordinates).  With head_dim 16 the kernel is bound by exp/softmax issue, not by the MMAs,
-// which is why the legacy warp-level mma.sync path is used here instead of a tensor-memory round trip.
+// keep base-`window_size` coordinates).  With head_dim 16 the kernel is bound by exp/softmax issue, not by the MMAs.  It
+// serves the windows the wgmma kernel (attn_tc.cu) has no schedule for (more than 352 tokens or more than 8 shift-mask
+// patterns) and, with B200_ATTN_HMMA=1, every window.
 constexpr int kAttKStride = 24;   // halfs per K row in smem (48 B: conflict-free b-fragment loads)
 
 __device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -641,12 +641,6 @@ __global__ void __launch_bounds__(256) head_conv_norm_nc8_kernel(HeadNormP p) {
 
 }  // namespace b200
 
-namespace b200 {
-int launch_head_conv_norm_tc(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res, int res_ctot,
-                             int res_coff, const float* res_stats, float slope, const float* weight, const float* bias, int Cout,
-                             void* y, int out_dtype, cudaStream_t st);
-}
-
 using namespace b200;
 
 extern "C" int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
@@ -657,17 +651,6 @@ extern "C" int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S,
   B200_REQUIRE(!res || (res_ctot % 8 == 0 && res_coff % 8 == 0 && res_coff + C <= res_ctot), "head_conv_norm_nc8: bad residual channel slice");
   B200_REQUIRE(res || !res_stats, "head_conv_norm_nc8: residual statistics without a residual");
   B200_REQUIRE(out_dtype == B200_DT_F16 || out_dtype == B200_DT_F32, "head_conv_norm_nc8: bad dtype");
-  {
-    // B200_HEAD_TC=1: tensor-core version (head_tc.cu) for the shapes it covers.  Off by default: both forms run at the same
-    // 4.1-4.4 TB/s on the C3 head (44.1 ms against 42.0 ms per volume) -- twelve concurrent 2 KB streams per tile, not the FMAs, set
-    // the pace -- so a larger MMA buys nothing here.
-    static const bool use_tc = std::getenv("B200_HEAD_TC") != nullptr;
-    if (use_tc) {
-      const int rc = launch_head_conv_norm_tc(x, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, slope, weight, bias, Cout, y,
-                                              out_dtype, (cudaStream_t)stream);
-      if (rc != B200_ERR_UNSUPPORTED) return rc;
-    }
-  }
   HeadNormP p{(const __half*)x, (const __half*)res, stats, res_stats, weight, bias, y, C, Cout, res_ctot, res_coff, S, eps, slope};
   dim3 grid(ceil_div(S, 256), N);
   const size_t smem = ((size_t)Cout * C + 4 * (size_t)C) * sizeof(float);

@@ -9,7 +9,9 @@ the whole network runs on fp16 channel-blocked ("NC8") buffers through the C ABI
   * Linear / 1x1x1 conv / ConvTranspose k2 s2: `b200_gemm_tc` (bias, GELU, residual, window-reverse scatter,
     2x upsample scatter fused in the epilogue);
   * LayerNorm + pad + cyclic shift + window partition: one gather kernel (`b200_layernorm_nc8`);
-  * windowed attention with relative-position bias and shift mask: `b200_window_attention_nc8`;
+  * windowed attention with relative-position bias and shift mask: `b200_window_attention_tc` (wgmma), or
+    `b200_window_attention_nc8` (mma.sync) for windows it has no schedule for (more than 352 tokens or more than 8 mask patterns)
+    and, with B200_ATTN_HMMA=1, for every window;
   * PatchMerging gather + LayerNorm, the single-channel stems and the output head: dedicated kernels.
 
 Skip concatenations are zero-copy: producers write straight into channel slices of the decoder's input buffer.
@@ -21,7 +23,6 @@ downsample "merging"/"mergingv2", use_v2 (the residual conv block in front of ev
 from __future__ import annotations
 
 import itertools
-import os
 from collections.abc import Sequence
 
 import numpy as np
@@ -299,7 +300,7 @@ class SwinUNETR(GraphedForward, nn.Module):
         if any((feature_size * 2**i) % h for i, h in enumerate(num_heads)) or any(d not in (8, 16, 24, 32, 48, 64) for d in head_dims):
             raise NotImplementedError(f"monai_b200 window attention supports head dimensions 8, 16, 24, 32, 48, 64 (got {head_dims})")
         self._tc_ok = feature_size % 48 == 0 and all(d == 16 for d in head_dims)
-        self.fp32_faithful = False   # set True (or B200_SWIN_FP32=1) to run fp32-storage generic kernels: <= 1e-3 of the fp32 reference
+        self.fp32_faithful = False   # set True to run fp32-storage generic kernels: <= 1e-3 of the fp32 reference
         nn_name = norm_name if isinstance(norm_name, str) else norm_name[0]
         if str(nn_name).lower() != "instance" or (not isinstance(norm_name, str) and norm_name[1].get("affine")):
             raise NotImplementedError("monai_b200 SwinUNETR implements norm_name='instance' (non-affine)")
@@ -412,7 +413,7 @@ class SwinUNETR(GraphedForward, nn.Module):
         folded = None
         if x_in_raw is not None:  # single input channel: direct stem kernels read the raw NCDHW window
             y1, st1 = K.conv_cin1_nc8(x_in_raw, blk.conv1.conv.weight, None, 3, 1, 1, want_stats=True)
-        elif K.RES_FOLD and hasattr(blk, "conv3") and cout <= 128 and cin_pad is None and blk.conv3.conv.bias is None:
+        elif hasattr(blk, "conv3") and cout <= 128 and cin_pad is None and blk.conv3.conv.bias is None:
             # conv3 (1x1x1 residual branch) reads the same input as conv1: one launch produces both tensors and both statistics
             y1, st1, y3f, st3f = K.conv3x3x3_tc(x, self._w3(blk.conv1.conv, key + ".c1", cin_pad), cin, cout, in_coff=in_coff, want_stats=True,
                                                 res_w=self._wlin(blk.conv3.conv.weight, key + ".c3", cin_pad))
@@ -467,6 +468,7 @@ class SwinUNETR(GraphedForward, nn.Module):
                 qkv, _ = K.gemm_tc(xw, wq, C, 3 * C, bias=bq)
                 att = K.window_attention_tc(qkv, C, blk.num_heads, nW, n, self._attn_bias(blk.attn, (bkey, tuple(dims), tuple(ws), tuple(ss)), n, tc), tc[0], tc[2])
             else:
+                # mma.sync attention: windows without a wgmma schedule (more than 352 tokens or more than 8 shift-mask patterns), or B200_ATTN_HMMA=1
                 qkv, _ = K.gemm_tc(xw, self._wlin(blk.attn.qkv.weight, bkey + ".qkv"), C, 3 * C, bias=blk.attn.qkv.bias)
                 att = K.window_attention_nc8(qkv, C, blk.num_heads, nW, n, blk.attn.scale, blk.attn.relative_position_bias_table, blk.attn.window_size,
                                              region if any(s > 0 for s in ss) else None)
@@ -507,7 +509,7 @@ class SwinUNETR(GraphedForward, nn.Module):
             raise ValueError(f"expected {self.in_channels} input channel(s), got {x_in.shape[1]}")
         if x_in.dtype not in (torch.float16, torch.float32):
             raise TypeError(f"SwinUNETR takes float16/float32 inputs, got {x_in.dtype}")
-        if not self._tc_ok or self.fp32_faithful or os.environ.get("B200_SWIN_FP32"):
+        if not self._tc_ok or self.fp32_faithful:
             return self._forward_direct(x_in)
         if x_in.dtype == torch.float32 and not getattr(self, "_warned_fp32", False):
             import warnings

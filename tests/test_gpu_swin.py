@@ -185,6 +185,21 @@ def test_window_attention_tcgen05_matches_reference_math(ws, n, nW, heads):
         assert err < 4e-3, (n, reg is None, err)
 
 
+def _conv_cin1_cuda_core(x, weight, bias, k, stride, pad, want_stats=False):
+    """b200_conv_cin1_nc8 called directly: the CUDA-core stem on shapes that K.conv_cin1_nc8 sends to the wgmma stem."""
+    N, _, D, H, W = x.shape
+    Cout = weight.shape[0]
+    out = K.NC8(N, Cout, tuple((s + 2 * pad - k) // stride + 1 for s in (D, H, W)), x.device)
+    stats = ws = None
+    if want_stats:
+        stats = torch.empty((N * Cout, 2), device=x.device, dtype=torch.float32)
+        ws = K._ws(L.load().b200_conv_cin1_nc8_workspace_bytes(N, D, H, W, Cout, k, stride, pad), x.device)
+    w32, b32 = weight.float().contiguous(), None if bias is None else bias.float().contiguous()
+    K._call("conv_cin1_nc8", L.ptr(x), L.dt(x), N, D, H, W, L.ptr(w32), L.ptr(b32), Cout, k, stride, pad, L.ptr(out.buf), out.C, 0,
+            L.ptr(stats), L.ptr(ws), L.stream_ptr(x.device))
+    return out, stats
+
+
 def test_instance_norm_statistics_are_deterministic():
     """The epilogue statistics never go through floating-point atomics: two runs give the same bits, and the values agree
     with a float64 reference (conv3x3x3_tc, gemm_tc with a 1x1x1 conv, the single-channel stems)."""
@@ -208,12 +223,8 @@ def test_instance_norm_statistics_are_deterministic():
     torch.testing.assert_close(r1[0].cpu().double().reshape(3, 48, 2)[..., 1], (ref1 * ref1).sum(dim=(2, 3, 4)), rtol=2e-3, atol=5e-2)
     u = torch.randn((3, 1, 12, 20, 24), generator=g).half().to(DEV)
     wc = torch.randn((48, 1, 3, 3, 3), generator=g).to(DEV) / 5
-    for force in (False, True):
-        K._FORCE_CUDA_CORE_STEM = force
-        try:
-            rs = [K.conv_cin1_nc8(u, wc, None, 3, 1, 1, want_stats=True)[1] for _ in range(3)]
-        finally:
-            K._FORCE_CUDA_CORE_STEM = False
+    for stem in (K.conv_cin1_nc8, _conv_cin1_cuda_core):
+        rs = [stem(u, wc, None, 3, 1, 1, want_stats=True)[1] for _ in range(3)]
         assert torch.equal(rs[0], rs[1]) and torch.equal(rs[0], rs[2])
         refc = F.conv3d(u.double().cpu(), wc.double().cpu(), padding=1)
         torch.testing.assert_close(rs[0].cpu().double().reshape(3, 48, 2)[..., 1], (refc * refc).sum(dim=(2, 3, 4)), rtol=3e-3, atol=5e-2)
@@ -223,23 +234,20 @@ def test_instance_norm_statistics_are_deterministic():
 def test_cin1_stem_and_head(force_cuda_core):
     g = torch.Generator().manual_seed(4)
     x = torch.randn((2, 1, 8, 10, 12), generator=g)
-    K._FORCE_CUDA_CORE_STEM = force_cuda_core   # False: wgmma stems for (3,1,1) and (2,2,0); True: CUDA-core kernel for all
-    try:
-        for k, s, p in [(3, 1, 1), (2, 2, 0), (1, 1, 0)]:
-            w, b = torch.randn((48, 1, k, k, k), generator=g) / k**1.5, torch.randn(48, generator=g)
-            ref = F.conv3d(x, w, b, stride=s, padding=p)
-            for xin in (x, x.half()):
-                y, st = K.conv_cin1_nc8(xin.to(DEV), w.to(DEV), b.to(DEV), k, s, p, want_stats=True)
-                assert _rel(K.unpack_nc8(y, dtype=torch.float32).cpu().numpy(), ref.numpy()) < 3e-3, (k, s, p, xin.dtype)
-                torch.testing.assert_close(st[:, 0].cpu(), ref.sum(dim=(2, 3, 4)).reshape(-1), rtol=2e-3, atol=3e-2)
-        # a volume that needs several tiles per axis and a partial last tile on every axis
-        xb = torch.randn((2, 1, 21, 37, 19), generator=g).half()
-        wb = torch.randn((32, 1, 3, 3, 3), generator=g) / 5
-        refb = F.conv3d(xb.float(), wb, padding=1)
-        yb, _ = K.conv_cin1_nc8(xb.to(DEV), wb.to(DEV), None, 3, 1, 1)
-        assert _rel(K.unpack_nc8(yb, dtype=torch.float32).cpu().numpy(), refb.numpy()) < 3e-3
-    finally:
-        K._FORCE_CUDA_CORE_STEM = False
+    stem = _conv_cin1_cuda_core if force_cuda_core else K.conv_cin1_nc8   # False: wgmma stems for (3,1,1) and (2,2,0)
+    for k, s, p in [(3, 1, 1), (2, 2, 0), (1, 1, 0)]:
+        w, b = torch.randn((48, 1, k, k, k), generator=g) / k**1.5, torch.randn(48, generator=g)
+        ref = F.conv3d(x, w, b, stride=s, padding=p)
+        for xin in (x, x.half()):
+            y, st = stem(xin.to(DEV), w.to(DEV), b.to(DEV), k, s, p, want_stats=True)
+            assert _rel(K.unpack_nc8(y, dtype=torch.float32).cpu().numpy(), ref.numpy()) < 3e-3, (k, s, p, xin.dtype)
+            torch.testing.assert_close(st[:, 0].cpu(), ref.sum(dim=(2, 3, 4)).reshape(-1), rtol=2e-3, atol=3e-2)
+    # a volume that needs several tiles per axis and a partial last tile on every axis
+    xb = torch.randn((2, 1, 21, 37, 19), generator=g).half()
+    wb = torch.randn((32, 1, 3, 3, 3), generator=g) / 5
+    refb = F.conv3d(xb.float(), wb, padding=1)
+    yb, _ = stem(xb.to(DEV), wb.to(DEV), None, 3, 1, 1)
+    assert _rel(K.unpack_nc8(yb, dtype=torch.float32).cpu().numpy(), refb.numpy()) < 3e-3
     h = torch.randn((2, 48, 4, 5, 6), generator=g).half()
     w, b = torch.randn((2, 48, 1, 1, 1), generator=g) / 7, torch.randn(2, generator=g)
     ref = F.conv3d(h.float(), w, b)
@@ -274,9 +282,9 @@ def test_fused_residual_tail_kernels():
     assert _rel(K.unpack_nc8(got_c).float().cpu().numpy(), ref_c.numpy()) < 3e-3
 
 
-def test_head_on_tensor_cores_many_tiles_and_classes():
-    """head_conv_norm_nc8 at C = 48 (with B200_HEAD_TC=1: wgmma per 128 voxels, head_tc.cu): 14 classes, several batch items, a
-    ragged last tile, fp16 and fp32 logits -- against torch fp32 (dynunet_block.py:104-111 + 247-267)."""
+def test_head_at_48_channels_and_14_classes():
+    """head_conv_norm_nc8 at C = 48: 14 classes, several batch items, a ragged last block, fp16 and fp32 logits -- against
+    torch fp32 (dynunet_block.py:104-111 + 247-267)."""
     g = torch.Generator().manual_seed(5)
     N, C, sp, CO = 3, 48, (9, 20, 23), 14
     y2 = (torch.randn((N, C, *sp), generator=g) * 1.3 + 0.2).half()
@@ -293,20 +301,6 @@ def test_head_on_tensor_cores_many_tiles_and_classes():
         assert r < 3e-3, (dt, r)
     again = K.head_conv_norm_nc8(y2n, st2, y3n, 0, st3, 0.01, 1e-5, w.to(DEV), b.to(DEV), out_dtype=torch.float16)
     assert torch.equal(again, got)
-
-
-def test_head_tensor_core_variant_in_a_subprocess():
-    """The opt-in wgmma form of the head (B200_HEAD_TC=1, read once per process) against the same references."""
-    import subprocess
-    import sys
-
-    if os.environ.get("B200_HEAD_TC"):
-        pytest.skip("already running with B200_HEAD_TC")
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-q", "-m", "gpu", "-p", "no:cacheprovider",
-                        "-k", "head_on_tensor_cores or fused_residual_tail"], env=dict(os.environ, B200_HEAD_TC="1"),
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    assert "2 passed" in r.stdout, r.stdout[-500:]
 
 
 def _build():
