@@ -665,9 +665,6 @@ def gemm_tc(
     return out, stats
 
 
-NORM_ON_LOAD = os.environ.get("B200_NORM_UNFUSED", "") == ""   # B200_NORM_UNFUSED=1: norm_act_nc8 pass between conv1 and conv2 (DESIGN.md §9)
-
-
 def mlp_fused_supported(C_: int, hidden: int) -> bool:
     return C_ == 48 and hidden == 192
 

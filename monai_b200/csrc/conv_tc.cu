@@ -183,6 +183,7 @@ __global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3
   static_assert(3 * kSA + 2 * kSB + 4 <= 48, "barrier block");
   float* s_stats = reinterpret_cast<float*>(bars + 48);  // [kStatRows][2*NT]
   float* s_stage = s_stats + Cfg::kStatRows * 2 * NT;    // [2 warpgroups][2][kStageFloats]
+  float* s_norm = s_stage + 2 * 2 * tc::kStageFloats;    // NORM: [Cin][2] (rstd, -mean * rstd) of one batch item
 
   const b200_conv_tc_desc& d = p.d;
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
@@ -314,46 +315,67 @@ __global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3
     if constexpr (RES) conv_stats_final(p.r, ws_r, NT, group_r, g, wid, lane);
   } else if constexpr (NORM) {
     // ===================== operand transform (warps 1-3): InstanceNorm + activation in place =====================
+    // Thread tt < kRowT * kHW owns voxel column px = tt % kHW of rows py = tt / kHW + kRowT * i of every plane of both chunk
+    // images: the column bounds test is one per tile, the row test one per row, and a warp's 32 vectors are contiguous.
+    // (rstd, -mean * rstd) of every input channel of the tile's batch item sit in a shared table, rebuilt only when the item
+    // changes (named barrier 1 of the 96 transform threads; the consumer warpgroups use ids 8 and 9).
+    constexpr int kRowT = 96 / kHW;                        // rows per pass
+    static_assert(kHH % kRowT == 0, "the rows of a plane split evenly into passes");
     const int tt = threadIdx.x - 32;                       // 0..95
-    constexpr int kVox = Cfg::kPlanes * kHH * kHW;         // 16-byte voxel vectors per chunk image
+    const int px = tt % kHW, py0 = tt / kHW;
+    const bool walker = tt < kRowT * kHW;
     const float invS = 1.f / ((float)d.D * (float)d.H * (float)d.W);
     const float slope = d.in_act == 1 ? d.in_slope : (d.in_act == 3 ? 0.f : 1.f), eps = d.in_eps;
     int sa = 0; uint32_t pa = 0;
+    int table_n = -1;
     for (long long t = blockIdx.x; t < p.e.total_tiles; t += gridDim.x) {
       const ConvTile c = conv_tile<BD>(p.e, t);
+      if (c.n != table_n) {
+        tc::named_bar(1, 96);          // every transform thread is done with the previous item's table
+        const float* st = p.in_stats + 2 * (long long)c.n * d.Cin;
+        for (int ch = tt; ch < d.Cin; ch += 96) {
+          // the expression and rounding of norm_act_nc8_kernel
+          const float sm = __ldg(st + 2 * ch), q = __ldg(st + 2 * ch + 1);
+          const float mean = sm * invS, var = fmaxf(q * invS - mean * mean, 0.f), rstd = 1.f / sqrtf(var + eps);
+          s_norm[2 * ch] = rstd; s_norm[2 * ch + 1] = -mean * rstd;
+        }
+        tc::named_bar(1, 96);
+        table_n = c.n;
+      }
+      const bool col_in = walker && (unsigned)(c.w0 - 1 + px) < (unsigned)d.W;
       for (int kc = 0; kc < num_kc; ++kc) {
         float sc[16], sh[16];
-        {
-          const float* st = p.in_stats + 2 * ((long long)c.n * d.Cin + kc * 16);
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float sm = __ldg(st + 2 * j), q = __ldg(st + 2 * j + 1);
-            const float mean = sm * invS, var = fmaxf(q * invS - mean * mean, 0.f), rstd = 1.f / sqrtf(var + eps);
-            sc[j] = rstd; sh[j] = -mean * rstd;
-          }
+        for (int j = 0; j < 16; ++j) {
+          const float2 v = reinterpret_cast<const float2*>(s_norm)[kc * 16 + j];
+          sc[j] = v.x; sh[j] = v.y;
         }
         tc::mbar_wait(&full_a[sa], pa);
-        uint8_t* img = smem_a + sa * Cfg::kABytes;
+        uint8_t* img = smem_a + sa * Cfg::kABytes + (py0 * kHW + px) * 16;
+        if (col_in) {
 #pragma unroll 2
-        for (int v = tt; v < 2 * kVox; v += 96) {
-          const int chunk = v >= kVox ? 1 : 0, vi = v - chunk * kVox;
-          const int pz = vi / (kHH * kHW), rem = vi - pz * (kHH * kHW), py = rem / kHW, px = rem - py * kHW;
-          const int gz = c.d0 - 1 + pz, gy = c.h0 - 1 + py, gx = c.w0 - 1 + px;
-          if ((unsigned)gz < (unsigned)d.D && (unsigned)gy < (unsigned)d.H && (unsigned)gx < (unsigned)d.W) {
-            uint4* ptr = reinterpret_cast<uint4*>(img + chunk * Cfg::kChunkBytes + vi * 16);
-            uint4 raw = *ptr;
-            __half2* h2 = reinterpret_cast<__half2*>(&raw);
+          for (int pz = 0; pz < Cfg::kPlanes; ++pz) {
+            if ((unsigned)(c.d0 - 1 + pz) >= (unsigned)d.D) continue;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float2 f = __half22float2(h2[j]);
-              const float s0 = chunk ? sc[8 + 2 * j] : sc[2 * j], s1 = chunk ? sc[9 + 2 * j] : sc[2 * j + 1];
-              const float o0 = chunk ? sh[8 + 2 * j] : sh[2 * j], o1 = chunk ? sh[9 + 2 * j] : sh[2 * j + 1];
-              const float a = fmaf(f.x, s0, o0), b = fmaf(f.y, s1, o1);
-              // one branch-free form for none / leaky-relu / relu: max(a, a * s) with s = 1 / slope / 0 (0 <= slope <= 1) returns
-              // exactly what `a >= 0 ? a : a * slope` returns
-              h2[j] = __floats2half2_rn(fmaxf(a, a * slope), fmaxf(b, b * slope));
+            for (int i = 0; i < kHH / kRowT; ++i) {
+              if ((unsigned)(c.h0 - 1 + py0 + kRowT * i) >= (unsigned)d.H) continue;
+#pragma unroll
+              for (int chunk = 0; chunk < 2; ++chunk) {
+                uint4* ptr = reinterpret_cast<uint4*>(img + chunk * Cfg::kChunkBytes + ((pz * kHH + kRowT * i) * kHW) * 16);
+                uint4 raw = *ptr;
+                __half2* h2 = reinterpret_cast<__half2*>(&raw);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  const float2 f = __half22float2(h2[j]);
+                  const float a = fmaf(f.x, sc[8 * chunk + 2 * j], sh[8 * chunk + 2 * j]);
+                  const float b = fmaf(f.y, sc[8 * chunk + 2 * j + 1], sh[8 * chunk + 2 * j + 1]);
+                  // one branch-free form for none / leaky-relu / relu: max(a, a * s) with s = 1 / slope / 0 (0 <= slope <= 1)
+                  // returns exactly what `a >= 0 ? a : a * slope` returns
+                  h2[j] = __floats2half2_rn(fmaxf(a, a * slope), fmaxf(b, b * slope));
+                }
+                *ptr = raw;
+              }
             }
-            *ptr = raw;
           }
         }
         tc::fence_proxy_async();       // generic-proxy stores -> visible to the wgmma operand reads
@@ -514,9 +536,11 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
   }
   dim3 grid((unsigned)std::min<long long>(p.e.total_tiles, num_sms()));
   auto kern = conv3x3x3_tc_kernel<NT, BD, NORM, RES>;
+  const int smem = Cfg::kSmemBytes + (NORM ? d.Cin * 8 : 0);   // NORM: the per-channel scale / shift table
+  B200_REQUIRE(smem <= 227 * 1024, "conv3x3x3_tc: Cin %d is too wide for the operand normalisation table", d.Cin);
   // per-device attribute: set on every call (cheap), so a second GPU in the same process works
-  B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  kern<<<grid, Cfg::kThreads, Cfg::kSmemBytes, c.st>>>(tmap, p);
+  B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p);
   B200_LAUNCH_CHECK("conv3x3x3_tc_kernel");
   if (c.stats) {
     const int rc = launch_stats_finish((const float*)c.ws, groups, R * kRows, NT, p.e.n_tiles, d.Cout, c.stats, c.st);

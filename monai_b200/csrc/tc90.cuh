@@ -120,6 +120,8 @@ __device__ __forceinline__ void wg_fence_acc(float* d) {
 }
 // named barrier of the 128 threads of one warpgroup (ids 8.. are free for this)
 __device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// named barrier of `threads` threads (a multiple of 32)
+__device__ __forceinline__ void named_bar(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 #include "wgmma_shapes.inc"
 

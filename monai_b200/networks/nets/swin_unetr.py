@@ -420,12 +420,8 @@ class SwinUNETR(GraphedForward, nn.Module):
             folded = (y3f, st3f)
         else:
             y1, st1 = K.conv3x3x3_tc(x, self._w3(blk.conv1.conv, key + ".c1", cin_pad), cin, cout, in_coff=in_coff, want_stats=True)
-        if K.NORM_ON_LOAD:
-            # norm1 + lrelu on conv2's operand load: y1 stays raw, no pass over the tensor in between
-            y2, st2 = K.conv3x3x3_tc(y1, self._w3(blk.conv2.conv, key + ".c2"), cout, cout, want_stats=True, in_norm=(st1, 1e-5, L.ACT_LEAKY, 0.01))
-        else:
-            K.norm_act_nc8(y1, cout, st1, act=L.ACT_LEAKY, slope=0.01, out=y1)
-            y2, st2 = K.conv3x3x3_tc(y1, self._w3(blk.conv2.conv, key + ".c2"), cout, cout, want_stats=True)
+        # norm1 + lrelu on conv2's operand load: y1 stays raw, no pass over the tensor in between
+        y2, st2 = K.conv3x3x3_tc(y1, self._w3(blk.conv2.conv, key + ".c2"), cout, cout, want_stats=True, in_norm=(st1, 1e-5, L.ACT_LEAKY, 0.01))
         if hasattr(blk, "conv3"):
             if x_in_raw is not None and x_in_raw.dtype == torch.float16 and blk.conv3.conv.bias is None and not defer_tail:
                 # one input channel: norm3(conv3(u)) is an affine function of u per channel -- no conv3 launch, no y3 tensor
