@@ -330,6 +330,14 @@ int b200_window_attention_tc_pack_bias(const float* table, int heads, int n, int
 int b200_window_attention_tc(const void* qkv, int N, int C, int heads, int nW, int n, const void* packed_bias,
                              const int32_t* sched, int ntypes, void* out, void* stream);
 
+/* Global multi-head self-attention of the ViT encoder (SABlock.forward, selfattention.py:170-217; no bias, no mask) on
+ * wgmma tensor cores, head_dim 64, any S >= 1:
+ *   qkv NC8 fp16 [N][3C/8][S][8], channel = (which * heads + h) * 64 + d  (which = q | k | v),
+ *   out NC8 fp16 [N][C/8][S][8],  channel = h * 64 + d.
+ * q must be PRE-SCALED by dim_head^-0.5 * log2(e) (fold it into the q rows of the qkv projection): the softmax runs in
+ * log2 units.  Deterministic.  C != 64 * heads: B200_ERR_UNSUPPORTED. */
+int b200_mhsa_tc(const void* qkv, int N, int C, int heads, long long S, void* out, void* stream);
+
 /* Convolution with ONE input channel straight from an NCDHW volume to NC8 (patch embedding k2 s2, the 3x3x3 stem of
  * UnetrBasicBlock and its 1x1x1 residual conv): weight float32 [Cout][1][k][k][k]; stats optional {sum,sumsq}. */
 long long b200_conv_cin1_nc8_workspace_bytes(int N, int D, int H, int W, int Cout, int k, int stride, int pad);

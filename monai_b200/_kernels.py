@@ -764,6 +764,23 @@ def window_attention_tc(qkv: NC8, Cc: int, heads: int, nW: int, n: int, packed_b
     return out
 
 
+def mhsa_tc(qkv: NC8, C_: int, heads: int) -> NC8:
+    """Global multi-head attention on wgmma (b200_mhsa_tc), head_dim 64: qkv NC8 [N][3C/8][S][8] with channels (q|k|v, head,
+    dim) -> NC8 [N][C/8][S][8].  q must be pre-scaled by dim_head^-0.5 * log2(e)."""
+    if qkv.C != 3 * C_:
+        raise ValueError(f"mhsa_tc: qkv has {qkv.C} channels, expected 3 * {C_}")
+    out = NC8(qkv.N, C_, qkv.sp, qkv.buf.device)
+    S = qkv.S
+    try:
+        _call("mhsa_tc", L.ptr(qkv.buf), qkv.N, C_, heads, S, L.ptr(out.buf), L.stream_ptr(qkv.buf.device),
+              flops=4.0 * qkv.N * heads * S * S * 64, nbytes=float(qkv.N * 4 * C_ * S * 2))
+    except RuntimeError as e:
+        if C_ != 64 * heads:   # B200_ERR_UNSUPPORTED: the kernel has no other head dimension, a bad argument of this call
+            raise ValueError(str(e)) from None
+        raise
+    return out
+
+
 ATTN_TC = not bool(os.environ.get("B200_ATTN_HMMA"))   # B200_ATTN_HMMA=1: mma.sync window_attention_nc8 for every window (DESIGN.md §9)
 LOG2E = 1.4426950408889634
 

@@ -120,6 +120,7 @@ SIGNATURES = {
     "b200_window_attention_tc_bias_bytes": (i64, [i32, i32, i32]),
     "b200_window_attention_tc_pack_bias": (i32, [vp, i32, i32, i32, i32, i32, vp, i32, vp, vp]),
     "b200_window_attention_tc": (i32, [vp, i32, i32, i32, i32, i32, vp, vp, i32, vp, vp]),
+    "b200_mhsa_tc": (i32, [vp, i32, i32, i32, i64, vp, vp]),
     "b200_patch_accumulate": (i32, [vp, i32, i64, i32, i32, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
     "b200_add_f32": (i32, [vp, vp, i64, vp]),
     "b200_patch_finalize": (i32, [vp, vp, i32, i64, vp]),
