@@ -314,12 +314,13 @@ int b200_patch_merge_ln_nc8(const void* x, int N, int C, int D, int H, int W, co
 int b200_window_attention_nc8(const void* qkv, int N, int C, int heads, int nW, int n, float scale, const float* table,
                               int ws0, int ws1, int ws2, const int32_t* region, void* out, void* stream);
 
-/* The same attention on wgmma tensor cores (n <= 352 tokens per window, head_dim 16): S = q k^T and the
- * relative-position bias + shift mask are BOTH accumulated by wgmma (the bias as an fp16 B operand resident in
- * shared memory, multiplied by an identity held in shared memory), online softmax in registers, P V runs on wgmma with the
- * probabilities as register operands and V read in place (MN-major operand).  Differences to b200_window_attention_nc8:
+/* The same attention on wgmma tensor cores (n <= 352 tokens per window, head_dim 16): S = q k^T is accumulated by wgmma
+ * onto the relative-position bias + shift mask (pre-packed in the accumulator's register order, resident in shared
+ * memory), online softmax in registers, P V runs on wgmma with the probabilities as register operands and V read in place
+ * (MN-major operand).  The packed bias is opaque to callers: size it with b200_window_attention_tc_bias_bytes.
+ * Differences to b200_window_attention_nc8:
  *   - q must be PRE-SCALED by scale * log2(e) (fold it into the q rows of the qkv projection): scores are in log2 units;
- *   - the bias table and the shift mask are pre-packed per (mask type, head, 128-row tile) with
+ *   - the bias table and the shift mask are pre-packed per (mask type, head, 192-row tile) with
  *     b200_window_attention_tc_pack_bias: region_types int32 [ntypes][n] holds ONE representative row of `region` per
  *     distinct mask pattern (NULL with ntypes = 1: no mask); ntypes <= 8;
  *   - sched int32 device array: count[8] (windows of each type), start[8] (offset of the type's window list),

@@ -6,7 +6,6 @@ sm_90a kernel reached through ctypes.  All functions require CUDA tensors.
 from __future__ import annotations
 
 import ctypes as C
-import os
 import weakref
 from typing import Sequence
 
@@ -744,7 +743,8 @@ def window_attention_tc_plan(region, nW: int, n: int):
 
 
 def window_attention_tc_pack_bias(table: torch.Tensor, heads: int, n: int, window: Sequence[int], region_types: torch.Tensor | None, ntypes: int) -> torch.Tensor:
-    """fp16 B-operand images of log2(e) * (relative-position bias + shift mask) per (mask type, head, 128-row tile)."""
+    """fp16 images of log2(e) * (relative-position bias + shift mask) per (mask type, head, 192-row tile), in the order of
+    the kernel's score accumulators."""
     tab = _f32c(table)
     nbytes = L.load().b200_window_attention_tc_bias_bytes(heads, n, ntypes)
     if nbytes < 0:
@@ -781,7 +781,6 @@ def mhsa_tc(qkv: NC8, C_: int, heads: int) -> NC8:
     return out
 
 
-ATTN_TC = not bool(os.environ.get("B200_ATTN_HMMA"))   # B200_ATTN_HMMA=1: mma.sync window_attention_nc8 for every window (DESIGN.md §9)
 LOG2E = 1.4426950408889634
 
 

@@ -3,23 +3,30 @@
 // Reference: WindowAttention.forward (monai/networks/nets/swin_unetr.py:509-532): per window of n <= 343 tokens and head
 // (head_dim 16):  softmax(q k^T * scale + relative_position_bias[:n,:n] + shift_mask) v.
 //
-// One persistent CTA per SM works on tiles = (window, head, 128-query row tile); two consumer warpgroups take 64 query rows
-// each and walk the keys in blocks of 32 (flash-attention style, online softmax):
-//   S[64 x 32] = Q K^T                          1 wgmma (SS form, K = 16 = the whole head)
-//              + I[64 x 64] * B'                4 wgmma (A = the identity rows of the warpgroup, resident in shared memory)
-// where B'[i][j] = log2(e) * (bias[i][j] + mask[i][j]) is an fp16 B operand that stays RESIDENT in shared memory: it depends
-// on (head, row tile, mask type) only, so tiles are scheduled (mask type, head, row tile)-major and a CTA reloads it a
-// handful of times per launch.  Adding the bias with the tensor core (1.0 * fp16 value into the fp32 accumulator: exact)
-// removes the per-element table lookup and mask test.  Padded keys carry B' = -30000 (P = 0).  Scores are in log2 units:
-// the caller folds scale * log2(e) into the q rows of the qkv projection.
-//   softmax: running row maximum m and row sum l in registers; P = 2^(S - m) rounded to fp16 -- the S accumulator fragment
-//            of a 32-key block is, packed to fp16 pairs, the register A operand of two K = 16 steps of
-//   O[64 x 16] += P V                           2 wgmma (RS form), V read in place as an MN-major B operand (NC8 rows are
-//            16-byte vectors of 8 dims); l sums the same fp16-rounded P values the MMA consumes;
+// With head_dim 16 the work is the n^2 exponentials (MUFU), not the MMAs, so the kernel is built to keep MUFU busy.
+// One persistent CTA per SM works on tiles = (window, head, 192-query row tile); three consumer warpgroups take 64 query rows
+// each and walk the keys in chunks of 64 (the last one may be 32; flash-attention style, online softmax):
+//   S[64 x 64] = B' + Q K^T                     1 wgmma (SS form, K = 16 = the whole head, scale-d = 1)
+// where B'[i][j] = log2(e) * (bias[i][j] + mask[i][j]) is loaded from shared memory straight into the accumulator
+// registers: the packed image is stored in the accumulator's fragment order (16 fp16 per thread per 32 keys, two 16-byte
+// vectors).  It depends on (mask type, head, row tile) only and stays RESIDENT in shared memory; tiles are scheduled
+// (mask type, head, window group, row tile, window) so that a CTA reloads it once per group of kAtGroup windows while
+// the K / V of those windows are still in L2 from the previous row tile.  Padded keys carry B' = -30000 (P = 0).  Scores
+// are in log2 units: the caller folds scale * log2(e) into the q rows of the qkv projection.
+//   softmax: running row maximum m (updated once per chunk) and row sum l in registers; P = 2^(S - m) rounded to fp16 --
+//            the S accumulator fragment, packed to fp16 pairs, is the register A operand of the K = 16 steps of
+//   O[64 x 16] += P V                           2-4 wgmma (RS form), V read in place as an MN-major B operand (NC8 rows
+//            are 16-byte vectors of 8 dims); l sums the same fp16-rounded P values the MMA consumes;
 //   epilogue: O / l -> fp16 NC8.
+// Software pipeline per warpgroup: the S MMA of chunk c+1 is in flight while the exponentials of chunk c run, and the PV
+// MMA of chunk c-1 retires only before O is rescaled (S and P are double-buffered in registers; P stays live until its
+// MMA retires).  A warp whose 16 query rows are all padding (rows >= n) takes part in the MMAs but issues no
+// exponential: its P is zero; a warpgroup whose 64 rows are all padding skips the tile.  Three consumer warpgroups (12
+// warps issuing exponentials, against 8 with two) hide the latency of each warp's max / shuffle / wgmma-wait chain.
 // Q, K, V tiles are 1-D bulk copies of NC8 rows (contiguous per 8-channel chunk); the producer runs up to two tiles ahead.
 //
-// Warp roles (384 threads): warp 0 = copy producer, warps 4-7 / 8-11 = the two consumer warpgroups.
+// Warp roles (512 threads): warp 0 = copy producer (warps 1-3 idle), warps 4-7 / 8-11 / 12-15 = the consumer warpgroups.
+// Warpgroup 0 gives its registers to the consumers (setmaxnreg 56 / 152).
 #include "common.cuh"
 #include "tc90.cuh"
 #include "../../include/monai_b200.h"
@@ -27,12 +34,18 @@
 namespace b200 {
 
 constexpr int kAtNPadMax = 352;                       // keys per window, padded (n <= 343 -> 352)
+constexpr int kAtWG = 3;                              // consumer warpgroups, 64 query rows each
+constexpr int kAtRows = 64 * kAtWG;                   // query rows per tile
+constexpr int kAtCT = 128 * kAtWG;                    // consumer threads
 constexpr int kAtKChunk = kAtNPadMax * 16;            // bytes of one 8-dim chunk of K / V in shared memory
-constexpr int kAtBiasBytes = 16 * kAtNPadMax * 16;    // 16 chunks of 8 query rows
-constexpr int kAtIdBytes = 16 * 2048;                 // identity operand image: [k chunk of 8][128 rows][16 B]
-constexpr int kAtQBytes = 2 * 2048, kAtKBytes = 2 * kAtKChunk, kAtVBytes = 2 * kAtKChunk;   // one buffer of each (two of each are kept)
-constexpr int kAtSmem = kAtBiasBytes + kAtIdBytes + 2 * (kAtQBytes + kAtKBytes + kAtVBytes) + 2 * 2 * tc::kStageFloats * 4 + 256 + 128;
+constexpr int kAtBiasBytes = kAtNPadMax * kAtCT;      // per 32 keys: every consumer thread x 16 fp16
+constexpr int kAtQBytes = 2 * kAtRows * 16, kAtKBytes = 2 * kAtKChunk, kAtVBytes = 2 * kAtKChunk;   // one buffer of each (two of each are kept)
+constexpr int kAtSmem = kAtBiasBytes + 2 * (kAtQBytes + kAtKBytes + kAtVBytes) + kAtWG * 2 * tc::kStageFloats * 4 + 256 + 128;
 constexpr float kAtPadBias = -30000.f;
+// windows per schedule group: the row tiles of a group run back to back on a CTA, so a window's K / V are read from HBM
+// about once; 132 CTAs x 8 windows x 22 KB (K and V of one head at n = 343) = 23 MB stays well inside the 50 MB L2,
+// and the 135 KB bias image is reloaded (from L2) once per 8 tiles
+constexpr int kAtGroup = 8;
 
 struct AttnTcParams {
   const __half* qkv; __half* out; const __half* bias; const int32_t* sched;
@@ -41,7 +54,8 @@ struct AttnTcParams {
 
 struct AttnTile { int ty, h, rt, b, w; };
 
-// flattened tile index -> (mask type, head, row tile, batch item, window); order: type, (head, row tile), batch, window
+// flattened tile index -> (mask type, head, row tile, batch item, window); order: type, head, group of kAtGroup (batch
+// item, window) pairs, row tile, pair within the group
 __device__ __forceinline__ AttnTile attn_decode(const AttnTcParams& p, long long f) {
   const int32_t* cnt = p.sched;
   const int32_t* start = p.sched + 8;
@@ -55,10 +69,23 @@ __device__ __forceinline__ AttnTile attn_decode(const AttnTcParams& p, long long
     f -= blk; ++t.ty;
   }
   const int c = cnt[t.ty];
-  const long long per = (long long)c * p.N;
-  const int hr = (int)(f / per);
-  const int l2 = (int)(f % per);
-  t.h = hr / p.nrt; t.rt = hr % p.nrt;
+  const int per = c * p.N;                              // (batch item, window) pairs of this type
+  const long long per_h = (long long)per * p.nrt;
+  t.h = (int)(f / per_h);
+  int r = (int)(f % per_h);
+  const int full = per / kAtGroup * kAtGroup;           // pairs in whole groups; the last group may be smaller
+  int l2;
+  if (r < full * p.nrt) {
+    const int grp = r / (kAtGroup * p.nrt);
+    r %= kAtGroup * p.nrt;
+    t.rt = r / kAtGroup;
+    l2 = grp * kAtGroup + r % kAtGroup;
+  } else {
+    r -= full * p.nrt;
+    const int rem = per - full;
+    t.rt = r / rem;
+    l2 = full + r % rem;
+  }
   t.b = l2 / c;
   t.w = win[start[t.ty] + l2 % c];
   return t;
@@ -78,27 +105,39 @@ __device__ __forceinline__ uint32_t exp2_pack(float a, float b, float m, float& 
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-constexpr int kAtThreads = 384;
+// 8 fp16 of the packed bias -> 8 accumulator registers
+__device__ __forceinline__ void bias_to_acc(const uint8_t* src, float* d) {
+  const uint4 v = *reinterpret_cast<const uint4*>(src);
+  const __half2* h = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 f = __half22float2(h[j]);
+    d[2 * j] = f.x; d[2 * j + 1] = f.y;
+  }
+}
+
+constexpr int kAtThreads = 128 * (kAtWG + 1);
 
 template <int NPAD>
 __global__ void __launch_bounds__(kAtThreads, 1) window_attention_tc_kernel(AttnTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = tc::align_smem128(smem_raw);   // keeps the shared address space (LDS/STS, not generic LD/ST)
-  uint8_t* s_bias = smem;
-  uint8_t* s_id = s_bias + kAtBiasBytes;              // identity operand image
-  uint8_t* s_q = s_id + kAtIdBytes;                   // [2 buffers][2 chunks][128 rows][16 B]
+  uint8_t* s_bias = smem;                             // [32-key block][2 halves][consumer thread][8 fp16]
+  uint8_t* s_q = s_bias + kAtBiasBytes;               // [2 buffers][2 chunks][kAtRows rows][16 B]
   uint8_t* s_k = s_q + 2 * kAtQBytes;                 // [2 buffers][2 chunks][n_pad keys][16 B]
   uint8_t* s_v = s_k + 2 * kAtKBytes;                 // [2 buffers][2 chunks: V dims 0-7, 8-15][n_pad keys][16 B]
-  float* s_stage = reinterpret_cast<float*>(s_v + 2 * kAtVBytes);   // [2 warpgroups][2][kStageFloats]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + 2 * 2 * tc::kStageFloats);
+  float* s_stage = reinterpret_cast<float*>(s_v + 2 * kAtVBytes);   // [kAtWG warpgroups][2][kStageFloats]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + kAtWG * 2 * tc::kStageFloats);
   uint64_t* qk_full = bars + 0;     // [2]  Q / K (+ bias) of a tile have landed in buffer b
-  uint64_t* qk_empty = bars + 2;    // [2]  the S MMAs that read buffer b are done (one arrival per consumer warpgroup)
+  uint64_t* qk_empty = bars + 2;    // [2]  the S MMAs (and bias loads) that read buffer b are done (one arrival per consumer warpgroup)
   uint64_t* v_full = bars + 4;      // [2]
   uint64_t* v_empty = bars + 6;     // [2]  the PV MMAs that read V buffer b are done
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-  // NPAD (keys per window, padded to a multiple of 32) is a template parameter: the key loop has a fixed trip count
+  // NPAD (keys per window, padded to a multiple of 32) is a template parameter: the key loop is fully unrolled
   constexpr int n_pad = NPAD;
+  constexpr int NB = NPAD / 32;          // 32-key blocks
+  constexpr int NC = (NB + 1) / 2;       // 64-key chunks (the last one has 32 keys when NB is odd)
   const int n = p.n;
   const long long T = (long long)p.nW * n;
   const long long total = (long long)p.N * p.nW * p.heads * p.nrt;
@@ -106,50 +145,48 @@ __global__ void __launch_bounds__(kAtThreads, 1) window_attention_tc_kernel(Attn
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&qk_full[i], 1); tc::mbar_init(&qk_empty[i], 2); tc::mbar_init(&v_full[i], 1); tc::mbar_init(&v_empty[i], 2);
+      tc::mbar_init(&qk_full[i], 1); tc::mbar_init(&qk_empty[i], kAtWG); tc::mbar_init(&v_full[i], 1); tc::mbar_init(&v_empty[i], kAtWG);
     }
     tc::fence_barrier_init();
   }
-  // zero the identity image and Q / K / V (rows the bulk copies never write must be finite)
+  // zero Q / K / V (rows the bulk copies never write must be finite)
   {
     const uint4 z = make_uint4(0, 0, 0, 0);
-    uint4* zq = reinterpret_cast<uint4*>(s_id);
-    const int nz = (kAtIdBytes + 2 * kAtQBytes + 2 * kAtKBytes + 2 * kAtVBytes) / 16;
+    uint4* zq = reinterpret_cast<uint4*>(s_q);
+    const int nz = (2 * kAtQBytes + 2 * kAtKBytes + 2 * kAtVBytes) / 16;
     for (int i = threadIdx.x; i < nz; i += blockDim.x) zq[i] = z;
-  }
-  __syncthreads();
-  {
-    __half* id = reinterpret_cast<__half*>(s_id);   // [k chunk of 8][row][8]: element (row r, k = r) = 1
-    for (int r = threadIdx.x; r < 128; r += blockDim.x) id[((r >> 3) * 128 + r) * 8 + (r & 7)] = __float2half_rn(1.f);
   }
   tc::fence_proxy_async();
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp < 4) {
+    // the copy producer needs few registers: warpgroup 0 hands them to the consumers, whose software pipeline keeps two S
+    // and two P fragments live (with the launch's 128 per thread ptxas would serialise the wgmma)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;\n" ::: "memory");
     // ===================== copy producer: runs up to two tiles ahead of the MMAs =====================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int last_combo = -1;
       int it = 0;
       for (long long f = lo; f < hi; ++f, ++it) {
         const AttnTile t = attn_decode(p, f);
         const int combo = (t.ty * p.heads + t.h) * p.nrt + t.rt;
-        const int rows = min(128, n - t.rt * 128);
+        const int rows = min(kAtRows, n - t.rt * kAtRows);
         const int b = it & 1;
         const uint32_t use = (uint32_t)((it >> 1) & 1);
         tc::mbar_wait(&qk_empty[b], use ^ 1u);                  // the S MMAs that read this buffer two tiles ago are done
         uint32_t bias_bytes = 0u;
         if (combo != last_combo) {
-          // the bias image is single-buffered: the S MMAs of the PREVIOUS tile (the other Q / K buffer) still read the old one
+          // the bias image is single-buffered: the consumers of the PREVIOUS tile (the other Q / K buffer) still read the old one
           if (it > 0) tc::mbar_wait(&qk_empty[b ^ 1], (uint32_t)(((it - 1) >> 1) & 1));
-          bias_bytes = (uint32_t)(16 * n_pad * 16);
+          bias_bytes = (uint32_t)(n_pad * kAtCT);
         }
         tc::mbar_arrive_expect_tx(&qk_full[b], bias_bytes + 2u * rows * 16u + 2u * n * 16u);
-        if (bias_bytes) tc::bulk_load(s_bias, p.bias + (long long)combo * (16 * n_pad * 8), bias_bytes, &qk_full[b]);
+        if (bias_bytes) tc::bulk_load(s_bias, p.bias + (long long)combo * (n_pad * kAtCT / 2), bias_bytes, &qk_full[b]);
         last_combo = combo;
         const __half* base = p.qkv + (long long)t.b * (3 * p.C8) * T * 8;
         const long long row0 = (long long)t.w * n;
         for (int c = 0; c < 2; ++c) {
-          tc::bulk_load(s_q + b * kAtQBytes + c * 2048, base + ((long long)(2 * t.h + c) * T + row0 + t.rt * 128) * 8, rows * 16, &qk_full[b]);
+          tc::bulk_load(s_q + b * kAtQBytes + c * kAtRows * 16, base + ((long long)(2 * t.h + c) * T + row0 + t.rt * kAtRows) * 8, rows * 16, &qk_full[b]);
           tc::bulk_load(s_k + b * kAtKBytes + c * kAtKChunk, base + ((long long)(p.C8 + 2 * t.h + c) * T + row0) * 8, n * 16, &qk_full[b]);
         }
         tc::mbar_wait(&v_empty[b], use ^ 1u);                   // the PV MMAs that read this V buffer two tiles ago are done
@@ -158,84 +195,125 @@ __global__ void __launch_bounds__(kAtThreads, 1) window_attention_tc_kernel(Attn
           tc::bulk_load(s_v + b * kAtVBytes + c * kAtKChunk, base + ((long long)(2 * p.C8 + 2 * t.h + c) * T + row0) * 8, n * 16, &v_full[b]);
       }
     }
-    __syncwarp();
-  } else if (warp >= 4) {
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 152;\n" ::: "memory");
     // ===================== consumers: warpgroup g owns query rows 64 g .. 64 g + 63 of every tile =====================
     const int g = (warp >> 2) - 1, wid = warp & 3;
-    const uint32_t q_a = tc::smem_u32(s_q), k_a = tc::smem_u32(s_k), v_a = tc::smem_u32(s_v), b_a = tc::smem_u32(s_bias),
-                   i_a = tc::smem_u32(s_id);
+    const int ct = threadIdx.x - 128;   // consumer thread: its slot in the packed bias
+    const uint32_t q_a = tc::smem_u32(s_q), k_a = tc::smem_u32(s_k), v_a = tc::smem_u32(s_v);
     float* stage = s_stage + g * 2 * tc::kStageFloats;
     int sl = 0;
     int it = 0;
     for (long long f = lo; f < hi; ++f, ++it) {
       const int b = it & 1;
       const uint32_t use = (uint32_t)((it >> 1) & 1);
+      const AttnTile t = attn_decode(p, f);
+      // all 16 rows of this warp are padding: no exponentials, P = 0 (the warp still takes part in the wgmma)
+      const bool dead = t.rt * kAtRows + 64 * g + 16 * wid >= n;
       float o[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = 0.f;
       float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // rows 16 wid + lane/4 and + 8 of the warpgroup
+      float s[2][32];          // S of chunks c (softmax) and c + 1 (MMA in flight)
+      uint32_t pa[2][4][4];    // P of chunks c (being built) and c - 1 (PV MMA in flight)
       tc::mbar_wait(&qk_full[b], use);
       tc::mbar_wait(&v_full[b], use);
-      const uint64_t qd = tc::make_desc_kmajor_noswz(q_a + b * kAtQBytes + g * 1024, 2048, 128);
-#pragma unroll 1
-      for (int kb = 0; kb < n_pad / 32; ++kb) {
-        // ---- S = Q K^T + I B' for 32 keys ----
-        float sc[16];
+      if (t.rt * kAtRows + 64 * g >= n) {
+        // all 64 rows of this warpgroup are padding (the last row tile of a small window): nothing to compute
+        if (wid == 0 && lane == 0) { tc::mbar_arrive(&qk_empty[b]); tc::mbar_arrive(&v_empty[b]); }
+        continue;
+      }
+      const uint64_t qd = tc::make_desc_kmajor_noswz(q_a + b * kAtQBytes + g * 1024, kAtRows * 16, 128);
+
+      // S(c) = B' + Q K^T for the keys of chunk c, committed as one wgmma group
+      auto issue_s = [&](auto cc) {
+        constexpr int c = decltype(cc)::value;
+        constexpr int nb = (2 * c + 1 < NB) ? 2 : 1;
+        float* sc = s[c & 1];
+#pragma unroll
+        for (int k2 = 0; k2 < nb; ++k2)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) bias_to_acc(s_bias + ((2 * c + k2) * 2 + hh) * (kAtCT * 16) + ct * 16, sc + 16 * k2 + 8 * hh);
         tc::wg_fence();
-        tc::Mma<32>::ss<0>(sc, qd, tc::make_desc_kmajor_noswz(k_a + b * kAtKBytes + kb * 32 * 16, kAtKChunk, 128), 0u);
-#pragma unroll
-        for (int s4 = 0; s4 < 4; ++s4) {
-          const int ks = 4 * g + s4;   // the identity rows of this warpgroup are non-zero in K steps 4g .. 4g+3 only
-          const uint64_t id_d = tc::make_desc_kmajor_noswz(i_a + ks * 4096 + g * 1024, 2048, 128);
-          const uint64_t bd = tc::make_desc_kmajor_noswz(b_a + (2 * ks) * n_pad * 16 + kb * 32 * 16, n_pad * 16, 128);
-          tc::Mma<32>::ss<0>(sc, id_d, bd, 1u);
-        }
+        const uint64_t kd = tc::make_desc_kmajor_noswz(k_a + b * kAtKBytes + c * 64 * 16, kAtKChunk, 128);
+        if constexpr (nb == 2) tc::Mma<64>::ss<0>(sc, qd, kd, 1u);
+        else tc::Mma<32>::ss<0>(sc, qd, kd, 1u);
         tc::wg_commit();
-        tc::wg_wait<0>();
-        tc::wg_fence_acc<16>(sc);
-        // ---- online softmax (the 4 lanes of a quad share a row) ----
-        float x0 = sc[0], x1 = sc[2];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          x0 = fmaxf(x0, fmaxf(sc[4 * i], sc[4 * i + 1]));
-          x1 = fmaxf(x1, fmaxf(sc[4 * i + 2], sc[4 * i + 3]));
+      };
+
+      issue_s(std::integral_constant<int, 0>{});
+      tc::static_for<0, NC>([&](auto cc) {
+        constexpr int c = decltype(cc)::value;
+        constexpr int nb = (2 * c + 1 < NB) ? 2 : 1;
+        constexpr int nv = 16 * nb;   // S registers of this chunk
+        // pending groups here: S(c), PV(c-1); after the next issue also S(c+1)
+        if constexpr (c + 1 < NC) {
+          issue_s(std::integral_constant<int, c + 1>{});
+          if constexpr (c == 0) tc::wg_wait<1>(); else tc::wg_wait<2>();
+        } else {
+          if constexpr (c == 0) tc::wg_wait<0>(); else tc::wg_wait<1>();
         }
-        x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 1)); x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 2));
-        x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 1)); x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 2));
-        const float n0 = fmaxf(m0, x0), n1 = fmaxf(m1, x1);
-        const float a0 = ex2(m0 - n0), a1 = ex2(m1 - n1);
-        m0 = n0; m1 = n1;
-        l0 *= a0; l1 *= a1;
+        float* sc = s[c & 1];
+        tc::wg_fence_acc<nv>(sc);
+        // ---- online softmax over the chunk (the 4 lanes of a quad share a row) ----
+        float a0 = 1.f, a1 = 1.f, ps0 = 0.f, ps1 = 0.f;
+        if (!dead) {
+          float x0 = sc[0], x1 = sc[2];
+#pragma unroll
+          for (int i = 0; i < nv / 4; ++i) {
+            x0 = fmaxf(x0, fmaxf(sc[4 * i], sc[4 * i + 1]));
+            x1 = fmaxf(x1, fmaxf(sc[4 * i + 2], sc[4 * i + 3]));
+          }
+          x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 1)); x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 2));
+          x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 1)); x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 2));
+          const float n0 = fmaxf(m0, x0), n1 = fmaxf(m1, x1);
+          a0 = ex2(m0 - n0); a1 = ex2(m1 - n1);
+          m0 = n0; m1 = n1;
+#pragma unroll
+          for (int kk = 0; kk < 2 * nb; ++kk) {
+            pa[c & 1][kk][0] = exp2_pack(sc[8 * kk + 0], sc[8 * kk + 1], m0, ps0);
+            pa[c & 1][kk][1] = exp2_pack(sc[8 * kk + 2], sc[8 * kk + 3], m1, ps1);
+            pa[c & 1][kk][2] = exp2_pack(sc[8 * kk + 4], sc[8 * kk + 5], m0, ps0);
+            pa[c & 1][kk][3] = exp2_pack(sc[8 * kk + 6], sc[8 * kk + 7], m1, ps1);
+          }
+        } else {
+#pragma unroll
+          for (int kk = 0; kk < 2 * nb; ++kk)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) pa[c & 1][kk][j] = 0u;
+        }
+        // ---- retire PV(c-1), then rescale O and l ----
+        if constexpr (c > 0) {
+          if constexpr (c + 1 < NC) tc::wg_wait<1>(); else tc::wg_wait<0>();
+          tc::wg_fence_acc<8>(o);
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(pa[(c - 1) & 1][kk][j])::"memory");   // A registers stay live until the wait
+        }
+        l0 = l0 * a0 + ps0; l1 = l1 * a1 + ps1;
 #pragma unroll
         for (int i = 0; i < 2; ++i) { o[4 * i] *= a0; o[4 * i + 1] *= a0; o[4 * i + 2] *= a1; o[4 * i + 3] *= a1; }
-        uint32_t pa[2][4];
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {
-          pa[kk][0] = exp2_pack(sc[8 * kk + 0], sc[8 * kk + 1], m0, l0);
-          pa[kk][1] = exp2_pack(sc[8 * kk + 2], sc[8 * kk + 3], m1, l1);
-          pa[kk][2] = exp2_pack(sc[8 * kk + 4], sc[8 * kk + 5], m0, l0);
-          pa[kk][3] = exp2_pack(sc[8 * kk + 6], sc[8 * kk + 7], m1, l1);
-        }
         // ---- O += P V (MN-major B: 8 keys x 16 B (8 dims) per core matrix, next 8 keys +128 B (LBO), next 8 dims +chunk (SBO)) ----
         tc::wg_fence();
 #pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {
-          const uint64_t vd = tc::make_desc_kmajor_noswz(v_a + b * kAtVBytes + (2 * kb + kk) * 256, 128, kAtKChunk);
-          tc::Mma<16>::rs<1>(o, pa[kk], vd, 1u);
+        for (int kk = 0; kk < 2 * nb; ++kk) {
+          const uint64_t vd = tc::make_desc_kmajor_noswz(v_a + b * kAtVBytes + (4 * c + kk) * 256, 128, kAtKChunk);
+          tc::Mma<16>::rs<1>(o, pa[c & 1][kk], vd, 1u);
         }
         tc::wg_commit();
-        tc::wg_wait<0>();
-        tc::wg_fence_acc<8>(o);
+      });
+      tc::wg_wait<0>();
+      tc::wg_fence_acc<8>(o);
 #pragma unroll
-        for (int kk = 0; kk < 2; ++kk)
+      for (int kk = 0; kk < 4; ++kk)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(pa[kk][j])::"memory");   // A registers stay live until the wait
-      }
+        for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(pa[(NC - 1) & 1][kk][j])::"memory");
       if (wid == 0 && lane == 0) { tc::mbar_arrive(&qk_empty[b]); tc::mbar_arrive(&v_empty[b]); }
       // ---- epilogue: O / l -> fp16 NC8 (one row and 8 dims per thread after the slice exchange) ----
       l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
       l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-      const float i0 = 1.f / l0, i1 = 1.f / l1;
+      const float i0 = dead ? 0.f : 1.f / l0, i1 = dead ? 0.f : 1.f / l1;
 #pragma unroll
       for (int i = 0; i < 2; ++i) { o[4 * i] *= i0; o[4 * i + 1] *= i0; o[4 * i + 2] *= i1; o[4 * i + 3] *= i1; }
       float* buf = stage + (sl & 1) * tc::kStageFloats;
@@ -244,8 +322,7 @@ __global__ void __launch_bounds__(kAtThreads, 1) window_attention_tc_kernel(Attn
       tc::wg_bar(8 + g);
       float v[8];
       tc::wg_read8(buf, wid, lane, v);
-      const AttnTile t = attn_decode(p, f);
-      const int r = t.rt * 128 + 64 * g + 32 * (wid & 1) + lane;
+      const int r = t.rt * kAtRows + 64 * g + 32 * (wid & 1) + lane;
       if (r < n) {
         const int dt = wid >> 1;
         __half* ob = p.out + (long long)t.b * p.C8 * T * 8 + ((long long)t.w * n + r) * 8;
@@ -259,22 +336,29 @@ __global__ void __launch_bounds__(kAtThreads, 1) window_attention_tc_kernel(Attn
   }
 }
 
-// B' operand images: [type][head][row tile][16 chunks of 8 query rows][n_pad keys][8] fp16 (see the header comment)
+// B' images in the S accumulator's fragment order: [type][head][row tile][32-key block][2 halves][kAtCT consumer threads][8]
+// fp16.  Consumer thread t = 128 g + 32 w + l (g < kAtWG) holds, for the 8-key column block i of a 32-key block, the values
+// (4 i + e) of the m64n32 accumulator: row 64 g + 16 w + l/4 (+ 8 for e >= 2), key 8 i + 2 (l % 4) + (e & 1); half hh
+// holds column blocks 2 hh and 2 hh + 1.
 __global__ void attn_bias_pack_kernel(const float* __restrict__ table, const int32_t* __restrict__ region, __half* __restrict__ out,
                                       int heads, int n, int n_pad, int nrt, int ntypes, int ws0, int ws1, int ws2) {
-  const long long total = (long long)ntypes * heads * nrt * 16 * n_pad * 8;
+  const long long total = (long long)ntypes * heads * nrt * n_pad * (kAtCT / 2);
   const int s1 = 2 * ws2 - 1, s0 = (2 * ws1 - 1) * s1;
   const int lin_c = (ws0 - 1) * s0 + (ws1 - 1) * s1 + (ws2 - 1);
+  const int nb = n_pad / 32;
   constexpr float kLog2e = 1.4426950408889634f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     long long r = i;
-    const int e = (int)(r % 8); r /= 8;
-    const int j = (int)(r % n_pad); r /= n_pad;
-    const int c = (int)(r % 16); r /= 16;
+    const int e8 = (int)(r % 8); r /= 8;
+    const int ct = (int)(r % kAtCT); r /= kAtCT;
+    const int hh = (int)(r % 2); r /= 2;
+    const int kb = (int)(r % nb); r /= nb;
     const int rt = (int)(r % nrt); r /= nrt;
     const int h = (int)(r % heads); r /= heads;
     const int ty = (int)r;
-    const int ig = rt * 128 + c * 8 + e;
+    const int v16 = 8 * hh + e8, cb = v16 >> 2, e = v16 & 3, l = ct & 31;
+    const int ig = rt * kAtRows + (ct >> 7) * 64 + ((ct >> 5) & 3) * 16 + (l >> 2) + (e >= 2 ? 8 : 0);
+    const int j = kb * 32 + cb * 8 + 2 * (l & 3) + (e & 1);
     float v;
     if (j >= n) v = kAtPadBias;
     else if (ig >= n) v = 0.f;
@@ -299,8 +383,8 @@ static bool attn_tc_shape_ok(int heads, int n, int ntypes) {
 
 extern "C" long long b200_window_attention_tc_bias_bytes(int heads, int n, int ntypes) {
   if (!attn_tc_shape_ok(heads, n, ntypes) || n > kAtNPadMax) return -1;
-  const int n_pad = (n + 31) / 32 * 32, nrt = (n + 127) / 128;
-  return (long long)ntypes * heads * nrt * 16 * n_pad * 16;
+  const int n_pad = (n + 31) / 32 * 32, nrt = (n + kAtRows - 1) / kAtRows;
+  return (long long)ntypes * heads * nrt * n_pad * kAtCT;
 }
 
 extern "C" int b200_window_attention_tc_pack_bias(const float* table, int heads, int n, int ws0, int ws1, int ws2,
@@ -309,8 +393,8 @@ extern "C" int b200_window_attention_tc_pack_bias(const float* table, int heads,
   B200_REQUIRE(attn_tc_shape_ok(heads, n, ntypes) && n <= kAtNPadMax, "window_attention_tc: unsupported shape (n = %d, types = %d)", n, ntypes);
   B200_REQUIRE(ws0 > 0 && ws1 > 0 && ws2 > 0 && n <= ws0 * ws1 * ws2, "window_attention_tc: window of %d tokens exceeds the module window", n);
   B200_REQUIRE(ntypes == 1 || region_types, "window_attention_tc_pack_bias: several mask types need their region rows");
-  const int n_pad = (n + 31) / 32 * 32, nrt = (n + 127) / 128;
-  const long long total = (long long)ntypes * heads * nrt * 16 * n_pad * 8;
+  const int n_pad = (n + 31) / 32 * 32, nrt = (n + kAtRows - 1) / kAtRows;
+  const long long total = (long long)ntypes * heads * nrt * n_pad * (kAtCT / 2);
   const int blocks = (int)std::min<long long>((total + 255) / 256, 8192);
   attn_bias_pack_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(table, region_types, (__half*)packed, heads, n, n_pad, nrt, ntypes, ws0, ws1, ws2);
   B200_LAUNCH_CHECK("attn_bias_pack_kernel");
@@ -325,7 +409,7 @@ extern "C" int b200_window_attention_tc(const void* qkv, int N, int C, int heads
   B200_REQUIRE(attn_tc_shape_ok(heads, n, ntypes) && n <= kAtNPadMax, "window_attention_tc: unsupported shape (n = %d, types = %d)", n, ntypes);
   AttnTcParams p;
   p.qkv = (const __half*)qkv; p.out = (__half*)out; p.bias = (const __half*)packed_bias; p.sched = sched;
-  p.N = N; p.C8 = C / 8; p.heads = heads; p.nW = nW; p.n = n; p.n_pad = (n + 31) / 32 * 32; p.nrt = (n + 127) / 128; p.ntypes = ntypes;
+  p.N = N; p.C8 = C / 8; p.heads = heads; p.nW = nW; p.n = n; p.n_pad = (n + 31) / 32 * 32; p.nrt = (n + kAtRows - 1) / kAtRows; p.ntypes = ntypes;
   const long long total = (long long)N * nW * heads * p.nrt;
   dim3 grid((unsigned)std::min<long long>(total, num_sms()));
   void (*kern)(AttnTcParams) = nullptr;

@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(256) layernorm8_nc8_kernel(const __half* __res
 // the MODULE window (the reference slices relative_position_index[:n, :n], swin_unetr.py:514-516, so clamped windows
 // keep base-`window_size` coordinates).  With head_dim 16 the kernel is bound by exp/softmax issue, not by the MMAs.  It
 // serves the windows the wgmma kernel (attn_tc.cu) has no schedule for (more than 352 tokens or more than 8 shift-mask
-// patterns) and, with B200_ATTN_HMMA=1, every window.
+// patterns).
 constexpr int kAttKStride = 24;   // halfs per K row in smem (48 B: conflict-free b-fragment loads)
 
 __device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {

@@ -10,8 +10,7 @@ the whole network runs on fp16 channel-blocked ("NC8") buffers through the C ABI
     2x upsample scatter fused in the epilogue);
   * LayerNorm + pad + cyclic shift + window partition: one gather kernel (`b200_layernorm_nc8`);
   * windowed attention with relative-position bias and shift mask: `b200_window_attention_tc` (wgmma), or
-    `b200_window_attention_nc8` (mma.sync) for windows it has no schedule for (more than 352 tokens or more than 8 mask patterns)
-    and, with B200_ATTN_HMMA=1, for every window;
+    `b200_window_attention_nc8` (mma.sync) for windows it has no schedule for (more than 352 tokens or more than 8 mask patterns);
   * PatchMerging gather + LayerNorm, the single-channel stems and the output head: dedicated kernels.
 
 Skip concatenations are zero-copy: producers write straight into channel slices of the decoder's input buffer.
@@ -356,13 +355,13 @@ class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
             src, region, nW, n, tc = self._plan(dims, ws, ss, dev)
             bkey = f"{key}.b{bi}"
             xw = K.layernorm_nc8(cur, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps, src=src, out_sp=(1, nW, n))
-            if K.ATTN_TC and tc is not None:
-                # tensor-core attention: bias + shift mask accumulated by the tensor core, scores in log2 units
+            if tc is not None:
+                # tensor-core attention: S accumulates onto the packed bias + shift mask, scores in log2 units
                 wq, bq = self._wqkv_scaled(blk.attn.qkv.weight, blk.attn.qkv.bias, C, blk.attn.scale, bkey)
                 qkv, _ = K.gemm_tc(xw, wq, C, 3 * C, bias=bq)
                 att = K.window_attention_tc(qkv, C, blk.num_heads, nW, n, self._attn_bias(blk.attn, (bkey, tuple(dims), tuple(ws), tuple(ss)), n, tc), tc[0], tc[2])
             else:
-                # mma.sync attention: windows without a wgmma schedule (more than 352 tokens or more than 8 shift-mask patterns), or B200_ATTN_HMMA=1
+                # mma.sync attention: windows without a wgmma schedule (more than 352 tokens or more than 8 shift-mask patterns)
                 qkv, _ = K.gemm_tc(xw, self._wlin(blk.attn.qkv.weight, bkey + ".qkv"), C, 3 * C, bias=blk.attn.qkv.bias)
                 att = K.window_attention_nc8(qkv, C, blk.num_heads, nW, n, blk.attn.scale, blk.attn.relative_position_bias_table, blk.attn.window_size,
                                              region if any(s > 0 for s in ss) else None)
