@@ -212,6 +212,11 @@ typedef struct b200_conv_tc_desc {
 long long b200_conv3x3x3_tc_workspace_bytes(const b200_conv_tc_desc* desc);
 int b200_conv3x3x3_tc(const b200_conv_tc_desc* desc, const void* x, const void* packed_w, const float* bias,
                       void* y, float* stats, void* workspace, void* stream);
+/* The same with an AFFINE operand normalisation (InstanceNorm3d(affine=True), dynunet_block.py:114-177): desc->in_stats is
+ * required and the kernel feeds act((x - mean) * rstd * in_gamma + in_beta), the fp16 values b200_norm_act_affine_nc8 would
+ * have stored.  in_gamma / in_beta: float32 device [Cin] (either may be NULL: 1 / 0).  Workspace as for b200_conv3x3x3_tc. */
+int b200_conv3x3x3_tc_affine(const b200_conv_tc_desc* desc, const float* in_gamma, const float* in_beta, const void* x,
+                             const void* packed_w, const float* bias, void* y, float* stats, void* workspace, void* stream);
 
 typedef struct b200_conv_gather_desc {
   int N, Cin, Cout;         /* Cin % 16 == 0; Cout arbitrary for NCDHW output, % 8 == 0 for NC8 output */
@@ -382,12 +387,25 @@ int b200_head_conv_nc8(const void* x, int N, int C, long long S, const float* we
 int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
                             int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
                             const float* bias, int Cout, void* y, int out_dtype, void* stream);
+/* The same with an affine InstanceNorm of x (DynUNet's last up block, dynunet_block.py:165-177): gamma / beta float32 device [C]
+ * (either may be NULL: 1 / 0). */
+int b200_head_conv_norm_affine_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
+                                   int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
+                                   const float* bias, int Cout, void* y, int out_dtype, const float* gamma, const float* beta,
+                                   void* stream);
 
 /* NC8 variant of b200_norm_act: y = act(instnorm(x) [+ instnorm?(res)]); act: 0 none, 1 leaky-relu(slope), 3 relu.
  * x / res / y are channel slices [coff, coff+C) of NC8 buffers with ctot channels. */
 int b200_norm_act_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats, float eps,
                       const void* res, int res_ctot, int res_coff, const float* res_stats, int act, float slope,
                       void* y, int y_ctot, int y_coff, void* stream);
+/* The same with affine InstanceNorms: y = act(instnorm(x) * gamma + beta [+ instnorm(res) * res_gamma + res_beta]) (UnetResBlock
+ * norm2 and norm3 with affine=True, dynunet_block.py:97-111).  Each parameter is float32 device [C] or NULL (1 / 0); gamma / beta
+ * need stats, res_gamma / res_beta need res_stats.  With all four NULL the output is bit-identical to b200_norm_act_nc8. */
+int b200_norm_act_affine_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats, float eps,
+                             const void* res, int res_ctot, int res_coff, const float* res_stats, int act, float slope,
+                             void* y, int y_ctot, int y_coff, const float* gamma, const float* beta, const float* res_gamma,
+                             const float* res_beta, void* stream);
 
 /* Same, for a residual block whose input has ONE channel (SwinUNETR encoder1): the residual branch
  * instnorm(conv1x1x1(u)) of UnetResBlock (dynunet_block.py:75-111) is evaluated analytically from the statistics of the

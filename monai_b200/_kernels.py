@@ -549,9 +549,11 @@ def conv3x3x3_tc(
     x: NC8, packed_w: torch.Tensor, Cin: int, Cout: int, in_coff: int = 0, bias: torch.Tensor | None = None,
     out: NC8 | None = None, out_coff: int = 0, want_stats: bool = False,
     in_norm: tuple[torch.Tensor, float, int, float] | None = None, res_w: torch.Tensor | None = None,
+    in_affine: tuple[torch.Tensor | None, torch.Tensor | None] | None = None,
 ):
     """3x3x3 / stride 1 / pad 1 convolution.  `in_norm` = (stats, eps, act, slope): x is the RAW output of the previous
     convolution and InstanceNorm + activation are applied on the operand load (no norm_act pass in between).
+    `in_affine` = (gamma, beta) of that InstanceNorm (affine=True; either may be None); it needs `in_norm`.
     `res_w` = gemm_tc_pack_weight image of a 1x1x1 convolution [Cout, Cin] of the SAME input: it is computed by the same launch
     and the call returns (out, stats, res_out, res_stats) instead of (out, stats)."""
     if out is None:
@@ -573,7 +575,13 @@ def conv3x3x3_tc(
             raise ValueError("conv3x3x3_tc: in_norm statistics must be a contiguous float32 [N*Cin, 2] tensor on the input's device")
         d.in_stats, d.in_eps, d.in_act, d.in_slope = L.ptr(st), float(eps), int(act), float(slope)
     ws = _ws(L.load().b200_conv3x3x3_tc_workspace_bytes(C.byref(d)), dev) if want_stats else None
-    _call("conv3x3x3_tc", C.byref(d), L.ptr(x.buf), L.ptr(packed_w), L.ptr(b32), L.ptr(out.buf), L.ptr(stats), L.ptr(ws), L.stream_ptr(dev),
+    if in_affine is not None and any(t is not None for t in in_affine):
+        if in_norm is None:
+            raise ValueError("conv3x3x3_tc: in_affine needs in_norm")
+        name, extra = "conv3x3x3_tc_affine", (L.ptr(_f32c(in_affine[0])), L.ptr(_f32c(in_affine[1])))
+    else:
+        name, extra = "conv3x3x3_tc", ()
+    _call(name, C.byref(d), *extra, L.ptr(x.buf), L.ptr(packed_w), L.ptr(b32), L.ptr(out.buf), L.ptr(stats), L.ptr(ws), L.stream_ptr(dev),
           flops=2.0 * x.N * x.S * Cin * Cout * (28 if res_w is not None else 27),
           nbytes=float(x.N * x.S * (Cin + Cout * (2 if res_w is not None else 1)) * 2) + _nb(packed_w))
     if res_w is not None:
@@ -599,13 +607,20 @@ def norm_act_cin1res_nc8(x: NC8, C_: int, stats: torch.Tensor, raw: torch.Tensor
 def norm_act_nc8(
     x: NC8, C_: int, stats: torch.Tensor | None, x_coff: int = 0, res: NC8 | None = None, res_coff: int = 0,
     res_stats: torch.Tensor | None = None, act: int = L.ACT_NONE, slope: float = 0.0, out: NC8 | None = None,
-    out_coff: int = 0, eps: float = 1e-5,
+    out_coff: int = 0, eps: float = 1e-5, gamma: torch.Tensor | None = None, beta: torch.Tensor | None = None,
+    res_gamma: torch.Tensor | None = None, res_beta: torch.Tensor | None = None,
 ) -> NC8:
+    """y = act(instnorm(x) [+ instnorm?(res)]) on NC8 channel slices; gamma / beta (res_gamma / res_beta) are the affine
+    parameters of x's (res's) InstanceNorm."""
     if out is None:
         out = NC8(x.N, C_, x.sp, x.buf.device)
-    _call("norm_act_nc8", L.ptr(x.buf), x.C, x_coff, x.N, C_, x.S, L.ptr(stats), eps, L.ptr(res.buf) if res is not None else None,
-            res.C if res is not None else 0, res_coff, L.ptr(res_stats), act, float(slope), L.ptr(out.buf), out.C, out_coff,
-            L.stream_ptr(x.buf.device))
+    affine = (gamma, beta, res_gamma, res_beta)
+    name, extra = "norm_act_nc8", ()
+    if any(t is not None for t in affine):
+        name, extra = "norm_act_affine_nc8", tuple(L.ptr(_f32c(t)) for t in affine)
+    _call(name, L.ptr(x.buf), x.C, x_coff, x.N, C_, x.S, L.ptr(stats), eps, L.ptr(res.buf) if res is not None else None,
+          res.C if res is not None else 0, res_coff, L.ptr(res_stats), act, float(slope), L.ptr(out.buf), out.C, out_coff, *extra,
+          L.stream_ptr(x.buf.device))
     return out
 
 
@@ -818,14 +833,19 @@ def head_conv_nc8(x: NC8, weight: torch.Tensor, bias: torch.Tensor | None, out_d
 
 
 def head_conv_norm_nc8(x: NC8, stats: torch.Tensor, res: NC8 | None, res_coff: int, res_stats: torch.Tensor | None, slope: float, eps: float,
-                       weight: torch.Tensor, bias: torch.Tensor | None, out_dtype: torch.dtype = torch.float16) -> torch.Tensor:
-    """logits = W * lrelu(instnorm(x) + instnorm?(res)) + b: the last residual block's tail fused into the 1x1x1 head."""
+                       weight: torch.Tensor, bias: torch.Tensor | None, out_dtype: torch.dtype = torch.float16,
+                       gamma: torch.Tensor | None = None, beta: torch.Tensor | None = None) -> torch.Tensor:
+    """logits = W * lrelu(instnorm(x) + instnorm?(res)) + b: the last block's tail fused into the 1x1x1 head; gamma / beta are
+    the affine parameters of x's InstanceNorm."""
     Cout = weight.shape[0]
     w32 = _f32c(weight)
     b32 = _f32c(bias)
     y = torch.empty((x.N, Cout, *x.sp), device=x.buf.device, dtype=out_dtype)
-    _call("head_conv_norm_nc8", L.ptr(x.buf), x.N, x.C, x.S, L.ptr(stats), float(eps), L.ptr(res.buf) if res is not None else None,
-          res.C if res is not None else 0, res_coff, L.ptr(res_stats), float(slope), L.ptr(w32), L.ptr(b32), Cout, L.ptr(y), L.dt(y),
+    name, extra = "head_conv_norm_nc8", ()
+    if gamma is not None or beta is not None:
+        name, extra = "head_conv_norm_affine_nc8", (L.ptr(_f32c(gamma)), L.ptr(_f32c(beta)))
+    _call(name, L.ptr(x.buf), x.N, x.C, x.S, L.ptr(stats), float(eps), L.ptr(res.buf) if res is not None else None,
+          res.C if res is not None else 0, res_coff, L.ptr(res_stats), float(slope), L.ptr(w32), L.ptr(b32), Cout, L.ptr(y), L.dt(y), *extra,
           L.stream_ptr(x.buf.device), nbytes=float(x.N * x.S * (x.C * (4 if res is not None else 2) + Cout * y.element_size())))
     return y
 

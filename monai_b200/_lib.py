@@ -96,6 +96,7 @@ SIGNATURES = {
     "b200_conv3x3x3_tc_pack_weight": (i32, [vp, i32, i32, vp, vp]),
     "b200_conv3x3x3_tc_workspace_bytes": (i64, [C.POINTER(ConvTcDesc)]),
     "b200_conv3x3x3_tc": (i32, [C.POINTER(ConvTcDesc), vp, vp, vp, vp, vp, vp, vp]),
+    "b200_conv3x3x3_tc_affine": (i32, [C.POINTER(ConvTcDesc), vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "b200_conv_gather_tc_weight_bytes": (i64, [C.POINTER(ConvGatherDesc)]),
     "b200_conv_gather_tc_pack_weight": (i32, [C.POINTER(ConvGatherDesc), vp, vp, vp]),
     "b200_conv_gather_tc_workspace_bytes": (i64, [C.POINTER(ConvGatherDesc)]),
@@ -127,7 +128,9 @@ SIGNATURES = {
     "b200_channel_post": (i32, [vp, i32, i32, i64, i32, f32, i32, vp, i32, vp]),
     "b200_head_conv_nc8": (i32, [vp, i32, i32, i64, vp, vp, i32, vp, i32, vp]),
     "b200_head_conv_norm_nc8": (i32, [vp, i32, i32, i64, vp, f32, vp, i32, i32, vp, f32, vp, vp, i32, vp, i32, vp]),
+    "b200_head_conv_norm_affine_nc8": (i32, [vp, i32, i32, i64, vp, f32, vp, i32, i32, vp, f32, vp, vp, i32, vp, i32, vp, vp, vp]),
     "b200_norm_act_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, i32, i32, vp, i32, f32, vp, i32, i32, vp]),
+    "b200_norm_act_affine_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, i32, i32, vp, i32, f32, vp, i32, i32, vp, vp, vp, vp, vp]),
     "b200_norm_act_cin1res_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, vp, vp, i32, f32, vp, i32, i32, vp]),
 }
 

@@ -142,9 +142,12 @@ struct ConvTcParams {
   const __half* w;      // packed
   ConvEpiP e;           // output stage (conv_epi.cuh)
   const float* in_stats;   // NORM: {sum, sumsq} per (n, input channel) of the raw input (see b200_conv_tc_desc.in_stats)
-  ConvEpiP r;              // RES: output stage of the folded 1x1x1 residual convolution
+  ConvEpiP r;             // RES: output stage of the folded 1x1x1 residual convolution
   const __half* res_w;     // RES: packed 1x1x1 weights (gemm_tc image: [nt][k16][khalf][NT/8][8][8])
 };
+// NORM: affine parameters of the operand's InstanceNorm, float32 [Cin] (NULL = 1 / 0); a kernel argument of its own, so that
+// ConvTcParams (and the code generated around it) is what it was before the affine variant existed
+struct ConvTcAffine { const float* gamma; const float* beta; };
 
 // Persistent, warp-specialised (384 threads, one CTA per SM): warp 0 = TMA producer, warps 4-7 and 8-11 = two consumer
 // warpgroups that run the wgmma chain of rows 0-63 / 64-127 of every tile with the fp32 accumulators in registers and then
@@ -153,8 +156,9 @@ struct ConvTcParams {
 //
 // NORM: the input is the RAW output of the previous convolution and InstanceNorm + activation
 // (monai/networks/blocks/dynunet_block.py:97-103: conv1 -> norm1 -> lrelu -> conv2) is applied on the operand load: warps 1-3
-// rewrite every staged halo tile in place -- y = act(x * rstd - mean * rstd), the exact expression and rounding of
-// norm_act_nc8_kernel, so the MMAs consume bit-identical fp16 operands -- between the TMA completion (full_a) and the MMAs
+// rewrite every staged halo tile in place -- y = act(x * scale + shift) with the (optionally affine) per-channel pair of
+// instnorm_scale_shift (stats.cuh), the exact expression and rounding of norm_act_nc8_kernel, so the MMAs consume
+// bit-identical fp16 operands -- between the TMA completion (full_a) and the MMAs
 // (ready_a).  Voxels outside the volume keep the TMA's zero fill: the convolution pads the NORMALISED tensor with zeros.
 // This removes one read and one write of the activation tensor per residual block.
 //
@@ -163,7 +167,8 @@ struct ConvTcParams {
 // halo tile (kh = kw = 1 of input plane o + 1) with the 1x1x1 weights into a second accumulator block, and the epilogue stores
 // both tensors with their statistics.  This deletes a launch that re-reads the 2 x C input tensor.
 template <int NT, int BD, bool NORM, bool RES>
-__global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3_tc_kernel(const __grid_constant__ CUtensorMap tmap, ConvTcParams p) {
+__global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3_tc_kernel(const __grid_constant__ CUtensorMap tmap, ConvTcParams p,
+                                                                                                  ConvTcAffine aff) {
   using Cfg = ConvTcCfg<NT, BD, RES>;
   static_assert(!(NORM && RES), "the residual fold is used by conv1, the operand normalisation by conv2");
   constexpr int kSA = Cfg::kSA, kSB = Cfg::kSB;
@@ -183,7 +188,7 @@ __global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3
   static_assert(3 * kSA + 2 * kSB + 4 <= 48, "barrier block");
   float* s_stats = reinterpret_cast<float*>(bars + 48);  // [kStatRows][2*NT]
   float* s_stage = s_stats + Cfg::kStatRows * 2 * NT;    // [2 warpgroups][2][kStageFloats]
-  float* s_norm = s_stage + 2 * 2 * tc::kStageFloats;    // NORM: [Cin][2] (rstd, -mean * rstd) of one batch item
+  float* s_norm = s_stage + 2 * 2 * tc::kStageFloats;    // NORM: [Cin][2] (scale, shift) of one batch item
 
   const b200_conv_tc_desc& d = p.d;
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
@@ -317,8 +322,9 @@ __global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3
     // ===================== operand transform (warps 1-3): InstanceNorm + activation in place =====================
     // Thread tt < kRowT * kHW owns voxel column px = tt % kHW of rows py = tt / kHW + kRowT * i of every plane of both chunk
     // images: the column bounds test is one per tile, the row test one per row, and a warp's 32 vectors are contiguous.
-    // (rstd, -mean * rstd) of every input channel of the tile's batch item sit in a shared table, rebuilt only when the item
-    // changes (named barrier 1 of the 96 transform threads; the consumer warpgroups use ids 8 and 9).
+    // (scale, shift) of every input channel of the tile's batch item -- (rstd, -mean * rstd), or with the affine parameters
+    // (gamma * rstd, beta - mean * rstd * gamma) -- sit in a shared table, rebuilt only when the item changes (named barrier 1
+    // of the 96 transform threads; the consumer warpgroups use ids 8 and 9).
     constexpr int kRowT = 96 / kHW;                        // rows per pass
     static_assert(kHH % kRowT == 0, "the rows of a plane split evenly into passes");
     const int tt = threadIdx.x - 32;                       // 0..95
@@ -333,12 +339,8 @@ __global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3
       if (c.n != table_n) {
         tc::named_bar(1, 96);          // every transform thread is done with the previous item's table
         const float* st = p.in_stats + 2 * (long long)c.n * d.Cin;
-        for (int ch = tt; ch < d.Cin; ch += 96) {
-          // the expression and rounding of norm_act_nc8_kernel
-          const float sm = __ldg(st + 2 * ch), q = __ldg(st + 2 * ch + 1);
-          const float mean = sm * invS, var = fmaxf(q * invS - mean * mean, 0.f), rstd = 1.f / sqrtf(var + eps);
-          s_norm[2 * ch] = rstd; s_norm[2 * ch + 1] = -mean * rstd;
-        }
+        for (int ch = tt; ch < d.Cin; ch += 96)   // the helper of norm_act_nc8_kernel: same (scale, shift) bits
+          reinterpret_cast<float2*>(s_norm)[ch] = instnorm_scale_shift(__ldg(st + 2 * ch), __ldg(st + 2 * ch + 1), invS, eps, aff.gamma, aff.beta, ch);
         tc::named_bar(1, 96);
         table_n = c.n;
       }
@@ -397,8 +399,13 @@ struct NormActNc8P {
   // single-channel residual branch evaluated analytically (see b200_norm_act_cin1res_nc8)
   const __half* raw; const float* raw_stats; const float* raw_w;
 };
+// affine parameters of the two InstanceNorms, float32 [C] (NULL = 1 / 0).  A kernel argument of its own: the non-affine
+// instantiation then compiles to the code (and the 48 registers) it had before the affine variant existed.
+struct NormAffineP { const float* gamma; const float* beta; const float* res_gamma; const float* res_beta; };
 
-__global__ void __launch_bounds__(256) norm_act_nc8_kernel(NormActNc8P p) {
+// AFFINE: apply the affine parameters `a` (a separate instantiation, so the non-affine launches keep their registers)
+template <bool AFFINE>
+__global__ void __launch_bounds__(256) norm_act_nc8_kernel(NormActNc8P p, NormAffineP a) {
   const int chunk = blockIdx.y, n = blockIdx.z;
   float sc[8], sh[8], rsc[8], rsh[8];
   const float invS = 1.f / (float)p.S;
@@ -407,14 +414,14 @@ __global__ void __launch_bounds__(256) norm_act_nc8_kernel(NormActNc8P p) {
     const int c = chunk * 8 + j;
     sc[j] = 1.f; sh[j] = 0.f; rsc[j] = 1.f; rsh[j] = 0.f;
     if (p.stats) {
-      const float s = p.stats[2 * (n * p.C + c)], q = p.stats[2 * (n * p.C + c) + 1];
-      const float mean = s * invS, var = fmaxf(q * invS - mean * mean, 0.f), rstd = 1.f / sqrtf(var + p.eps);
-      sc[j] = rstd; sh[j] = -mean * rstd;
+      const float2 k = instnorm_scale_shift(p.stats[2 * (n * p.C + c)], p.stats[2 * (n * p.C + c) + 1], invS, p.eps,
+                                            AFFINE ? a.gamma : nullptr, AFFINE ? a.beta : nullptr, c);
+      sc[j] = k.x; sh[j] = k.y;
     }
     if (p.res_stats) {
-      const float s = p.res_stats[2 * (n * p.C + c)], q = p.res_stats[2 * (n * p.C + c) + 1];
-      const float mean = s * invS, var = fmaxf(q * invS - mean * mean, 0.f), rstd = 1.f / sqrtf(var + p.eps);
-      rsc[j] = rstd; rsh[j] = -mean * rstd;
+      const float2 k = instnorm_scale_shift(p.res_stats[2 * (n * p.C + c)], p.res_stats[2 * (n * p.C + c) + 1], invS, p.eps,
+                                            AFFINE ? a.res_gamma : nullptr, AFFINE ? a.res_beta : nullptr, c);
+      rsc[j] = k.x; rsh[j] = k.y;
     }
     if (p.raw) {
       // residual = instnorm(w * u) of a 1-channel input u: mean = w mu, var = w^2 sigma^2  =>  alpha u + beta
@@ -500,7 +507,10 @@ struct ConvTcGeom {
 };
 
 // what a launch needs beyond the operands: mode 0 = run, mode 1 = only report the statistics workspace size
-struct ConvTcCall { const void* x; const void* w; const float* bias; void* y; float* stats; void* ws; cudaStream_t st; long long ws_bytes; int query; };
+struct ConvTcCall {
+  const void* x; const void* w; const float* bias; void* y; float* stats; void* ws; cudaStream_t st; long long ws_bytes; int query;
+  const float* in_gamma; const float* in_beta;   // NORM: affine parameters of the operand normalisation (NULL = non-affine)
+};
 
 template <int NT, int BD, bool NORM, bool RES = false>
 static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
@@ -540,7 +550,7 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
   B200_REQUIRE(smem <= 227 * 1024, "conv3x3x3_tc: Cin %d is too wide for the operand normalisation table", d.Cin);
   // per-device attribute: set on every call (cheap), so a second GPU in the same process works
   B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p);
+  kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, ConvTcAffine{c.in_gamma, c.in_beta});
   B200_LAUNCH_CHECK("conv3x3x3_tc_kernel");
   if (c.stats) {
     const int rc = launch_stats_finish((const float*)c.ws, groups, R * kRows, NT, p.e.n_tiles, d.Cout, c.stats, c.st);
@@ -602,27 +612,43 @@ static int conv_tc_dispatch(const b200_conv_tc_desc& d, ConvTcCall& c) {
 
 extern "C" long long b200_conv3x3x3_tc_workspace_bytes(const b200_conv_tc_desc* desc) {
   if (!desc) return -1;
-  ConvTcCall c{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1};
+  ConvTcCall c{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1, nullptr, nullptr};
   if (conv_tc_dispatch(*desc, c)) return -1;
   return c.ws_bytes;
 }
 
-extern "C" int b200_conv3x3x3_tc(const b200_conv_tc_desc* desc, const void* x, const void* packed_w, const float* bias,
-                                 void* y, float* stats, void* workspace, void* stream) {
+static int conv3x3x3_tc_run(const b200_conv_tc_desc* desc, const float* in_gamma, const float* in_beta, const void* x, const void* packed_w,
+                            const float* bias, void* y, float* stats, void* workspace, void* stream) {
   B200_REQUIRE(desc && x && packed_w && y, "conv3x3x3_tc: null pointer");
   B200_REQUIRE(!(stats || (desc && desc->res_stats)) || workspace, "conv3x3x3_tc: statistics need the workspace of b200_conv3x3x3_tc_workspace_bytes()");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
                (reinterpret_cast<uintptr_t>(packed_w) & 15) == 0, "conv3x3x3_tc: pointers must be 16-byte aligned");
-  ConvTcCall c{x, packed_w, bias, y, stats, workspace, (cudaStream_t)stream, 0, 0};
+  B200_REQUIRE(desc->in_stats || !(in_gamma || in_beta), "conv3x3x3_tc: affine parameters of the operand normalisation without in_stats");
+  ConvTcCall c{x, packed_w, bias, y, stats, workspace, (cudaStream_t)stream, 0, 0, in_gamma, in_beta};
   return conv_tc_dispatch(*desc, c);
 }
 
-extern "C" int b200_norm_act_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats,
-                                 float eps, const void* res, int res_ctot, int res_coff, const float* res_stats, int act,
-                                 float slope, void* y, int y_ctot, int y_coff, void* stream) {
+extern "C" int b200_conv3x3x3_tc(const b200_conv_tc_desc* desc, const void* x, const void* packed_w, const float* bias,
+                                 void* y, float* stats, void* workspace, void* stream) {
+  return conv3x3x3_tc_run(desc, nullptr, nullptr, x, packed_w, bias, y, stats, workspace, stream);
+}
+
+extern "C" int b200_conv3x3x3_tc_affine(const b200_conv_tc_desc* desc, const float* in_gamma, const float* in_beta, const void* x,
+                                        const void* packed_w, const float* bias, void* y, float* stats, void* workspace, void* stream) {
+  return conv3x3x3_tc_run(desc, in_gamma, in_beta, x, packed_w, bias, y, stats, workspace, stream);
+}
+
+// y = act(instnorm(x) [+ instnorm?(res)]) with optional affine parameters per norm: the body of b200_norm_act_nc8 and
+// b200_norm_act_affine_nc8
+static int norm_act_nc8_launch(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats, float eps,
+                               const void* res, int res_ctot, int res_coff, const float* res_stats, int act, float slope, void* y,
+                               int y_ctot, int y_coff, const float* gamma, const float* beta, const float* res_gamma,
+                               const float* res_beta, void* stream) {
   B200_REQUIRE(x && y, "norm_act_nc8: null pointer");
   B200_REQUIRE(C % 8 == 0 && x_ctot % 8 == 0 && x_coff % 8 == 0 && y_ctot % 8 == 0 && y_coff % 8 == 0, "norm_act_nc8: channels must be multiples of 8");
   B200_REQUIRE(act == 0 || act == 1 || act == 3, "norm_act_nc8: activation must be none, leaky-relu or relu");
+  B200_REQUIRE(stats || !(gamma || beta), "norm_act_nc8: affine parameters without statistics");
+  B200_REQUIRE(res_stats || !(res_gamma || res_beta), "norm_act_nc8: residual affine parameters without residual statistics");
   if ((long long)N * C * S == 0) return B200_OK;
   NormActNc8P p;
   p.x = (const __half*)x; p.y = (__half*)y; p.res = (const __half*)res; p.C = C;
@@ -631,9 +657,26 @@ extern "C" int b200_norm_act_nc8(const void* x, int x_ctot, int x_coff, int N, i
   p.raw = nullptr; p.raw_stats = nullptr; p.raw_w = nullptr;
   long long want = (long long)num_sms() * 16 / ((long long)N * (C / 8)) + 1;
   dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(want, (S + 255) / 256)), C / 8, N);
-  norm_act_nc8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
+  const NormAffineP a{gamma, beta, res_gamma, res_beta};
+  if (gamma || beta || res_gamma || res_beta) norm_act_nc8_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
+  else norm_act_nc8_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
   B200_LAUNCH_CHECK("norm_act_nc8_kernel");
   return B200_OK;
+}
+
+extern "C" int b200_norm_act_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats,
+                                 float eps, const void* res, int res_ctot, int res_coff, const float* res_stats, int act,
+                                 float slope, void* y, int y_ctot, int y_coff, void* stream) {
+  return norm_act_nc8_launch(x, x_ctot, x_coff, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, act, slope, y, y_ctot, y_coff,
+                             nullptr, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int b200_norm_act_affine_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats,
+                                        float eps, const void* res, int res_ctot, int res_coff, const float* res_stats, int act,
+                                        float slope, void* y, int y_ctot, int y_coff, const float* gamma, const float* beta,
+                                        const float* res_gamma, const float* res_beta, void* stream) {
+  return norm_act_nc8_launch(x, x_ctot, x_coff, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, act, slope, y, y_ctot, y_coff,
+                             gamma, beta, res_gamma, res_beta, stream);
 }
 
 extern "C" int b200_norm_act_cin1res_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats,
@@ -650,7 +693,7 @@ extern "C" int b200_norm_act_cin1res_nc8(const void* x, int x_ctot, int x_coff, 
   p.raw = (const __half*)raw; p.raw_stats = raw_stats; p.raw_w = raw_weight;
   long long want = (long long)num_sms() * 16 / ((long long)N * (C / 8)) + 1;
   dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(want, (S + 255) / 256)), C / 8, N);
-  norm_act_nc8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
+  norm_act_nc8_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(p, NormAffineP{nullptr, nullptr, nullptr, nullptr});
   B200_LAUNCH_CHECK("norm_act_nc8_kernel");
   return B200_OK;
 }

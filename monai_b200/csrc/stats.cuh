@@ -47,4 +47,18 @@ inline long long stats_partial_bytes(long long groups, int R, int NT, int rows_p
 // stats[(n*Cout + nt*NT + col)*2 + {0,1}] = sum over the `rows` (= R * rows_per_cta) partial rows of group (n, nt), fixed order, fp64.
 int launch_stats_finish(const float* partials, long long groups, int rows, int NT, int n_tiles, int Cout, float* stats, cudaStream_t st);
 
+// InstanceNorm of channel c as one multiply-add, y = x * scale + shift, from its {sum, sumsq} over S voxels (invS = 1 / S).
+// Every NC8 consumer of the statistics (norm_act_nc8_kernel, the operand table of conv3x3x3_tc, head_conv_norm_nc8_kernel)
+// calls this, so a fused and an unfused normalisation produce the same fp16 values.  gamma / beta (float32 [C], either may be
+// NULL) are the affine parameters: (gamma * rstd, beta - mean * rstd * gamma), as b200_norm_act computes them; with both NULL
+// the pair is (rstd, -mean * rstd).
+__device__ __forceinline__ float2 instnorm_scale_shift(float sum, float sumsq, float invS, float eps, const float* gamma,
+                                                       const float* beta, int c) {
+  const float mean = sum * invS, var = fmaxf(sumsq * invS - mean * mean, 0.f), rstd = 1.f / sqrtf(var + eps);
+  if (!gamma && !beta) return make_float2(rstd, -mean * rstd);
+  const float g = gamma ? __ldg(gamma + c) : 1.f, b = beta ? __ldg(beta + c) : 0.f;
+  // explicit roundings: the shift is the same float wherever the helper is inlined (no site-dependent FMA contraction)
+  return make_float2(__fmul_rn(rstd, g), __fsub_rn(b, __fmul_rn(__fmul_rn(mean, rstd), g)));
+}
+
 }  // namespace b200

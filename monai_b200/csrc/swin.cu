@@ -566,13 +566,15 @@ __global__ void __launch_bounds__(256) head_conv_nc8_kernel(const __half* __rest
     if (o < Cout) io<TO>::st(y + ((long long)n * Cout + o) * S + r, acc[o]);
 }
 
-// Output head fused with the tail of the last residual block (UnetResBlock.forward, dynunet_block.py:97-111, followed by
-// UnetOutBlock): y = W * lrelu(instnorm(x) + instnorm?(res)) + b.  The normalised activation never goes to HBM.
+// Output head fused with the tail of the last residual or basic block (UnetResBlock / UnetBasicBlock.forward,
+// dynunet_block.py:97-111 / 165-177, followed by UnetOutBlock): y = W * lrelu(instnorm(x) + instnorm?(res)) + b, x's norm
+// optionally affine.  The normalised activation never goes to HBM.
 struct HeadNormP {
   const __half* x; const __half* res; const float* stats; const float* res_stats; const float* wgt; const float* bias; void* y;
   int C, Cout, res_ctot, res_coff;
   long long S;
   float eps, slope;
+  const float* gamma; const float* beta;   // affine parameters of x's InstanceNorm, float32 [C] (NULL = non-affine)
 };
 
 // CO = compile-time bound on the output channels (registers and FMAs are spent on CO, not on the ABI maximum of 16)
@@ -587,15 +589,13 @@ __global__ void __launch_bounds__(256) head_conv_norm_nc8_kernel(HeadNormP p) {
   for (int i = threadIdx.x; i < p.Cout * p.C; i += blockDim.x) s_hn[i] = p.wgt[i];
   const float invS = 1.f / (float)p.S;
   for (int c = threadIdx.x; c < p.C; c += blockDim.x) {
-    // same statistics arithmetic as norm_act_nc8_kernel
-    const float s = p.stats[2 * (n * p.C + c)], q = p.stats[2 * (n * p.C + c) + 1];
-    const float mean = s * invS, var = fmaxf(q * invS - mean * mean, 0.f), rstd = 1.f / sqrtf(var + p.eps);
-    s_sc[c] = rstd; s_sh[c] = -mean * rstd;
+    // the helper of norm_act_nc8_kernel: same (scale, shift) bits
+    const float2 k = instnorm_scale_shift(p.stats[2 * (n * p.C + c)], p.stats[2 * (n * p.C + c) + 1], invS, p.eps, p.gamma, p.beta, c);
+    s_sc[c] = k.x; s_sh[c] = k.y;
     float rsc = 1.f, rsh = 0.f;
     if (p.res_stats) {
-      const float rs = p.res_stats[2 * (n * p.C + c)], rq = p.res_stats[2 * (n * p.C + c) + 1];
-      const float rmean = rs * invS, rvar = fmaxf(rq * invS - rmean * rmean, 0.f), rrstd = 1.f / sqrtf(rvar + p.eps);
-      rsc = rrstd; rsh = -rmean * rrstd;
+      const float2 r = instnorm_scale_shift(p.res_stats[2 * (n * p.C + c)], p.res_stats[2 * (n * p.C + c) + 1], invS, p.eps, nullptr, nullptr, c);
+      rsc = r.x; rsh = r.y;
     }
     s_rsc[c] = rsc; s_rsh[c] = rsh;
   }
@@ -643,15 +643,17 @@ __global__ void __launch_bounds__(256) head_conv_norm_nc8_kernel(HeadNormP p) {
 
 using namespace b200;
 
-extern "C" int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
-                                       int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
-                                       const float* bias, int Cout, void* y, int out_dtype, void* stream) {
+// the body of b200_head_conv_norm_nc8 and b200_head_conv_norm_affine_nc8
+static int head_conv_norm_nc8_launch(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
+                                     int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
+                                     const float* bias, int Cout, void* y, int out_dtype, const float* gamma, const float* beta,
+                                     void* stream) {
   B200_REQUIRE(x && y && weight && stats, "head_conv_norm_nc8: null pointer");
   B200_REQUIRE(C % 8 == 0 && Cout >= 1 && Cout <= 16, "head_conv_norm_nc8: C must be a multiple of 8 and Cout <= 16 (got %d, %d)", C, Cout);
   B200_REQUIRE(!res || (res_ctot % 8 == 0 && res_coff % 8 == 0 && res_coff + C <= res_ctot), "head_conv_norm_nc8: bad residual channel slice");
   B200_REQUIRE(res || !res_stats, "head_conv_norm_nc8: residual statistics without a residual");
   B200_REQUIRE(out_dtype == B200_DT_F16 || out_dtype == B200_DT_F32, "head_conv_norm_nc8: bad dtype");
-  HeadNormP p{(const __half*)x, (const __half*)res, stats, res_stats, weight, bias, y, C, Cout, res_ctot, res_coff, S, eps, slope};
+  HeadNormP p{(const __half*)x, (const __half*)res, stats, res_stats, weight, bias, y, C, Cout, res_ctot, res_coff, S, eps, slope, gamma, beta};
   dim3 grid(ceil_div(S, 256), N);
   const size_t smem = ((size_t)Cout * C + 4 * (size_t)C) * sizeof(float);
   B200_REQUIRE(smem <= 48 * 1024, "head_conv_norm_nc8: C too large (%d)", C);
@@ -665,6 +667,21 @@ extern "C" int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S,
 #undef LHN
   B200_LAUNCH_CHECK("head_conv_norm_nc8_kernel");
   return B200_OK;
+}
+
+extern "C" int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
+                                       int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
+                                       const float* bias, int Cout, void* y, int out_dtype, void* stream) {
+  return head_conv_norm_nc8_launch(x, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, slope, weight, bias, Cout, y, out_dtype,
+                                   nullptr, nullptr, stream);
+}
+
+extern "C" int b200_head_conv_norm_affine_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
+                                              int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
+                                              const float* bias, int Cout, void* y, int out_dtype, const float* gamma,
+                                              const float* beta, void* stream) {
+  return head_conv_norm_nc8_launch(x, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, slope, weight, bias, Cout, y, out_dtype,
+                                   gamma, beta, stream);
 }
 
 extern "C" int b200_layernorm_nc8(const void* x, int N, int C, long long S_in, const int32_t* src, long long S_out,
