@@ -1,13 +1,23 @@
-"""Pieces shared by the tensor-core forwards (SwinUNETR, UNETR, DynUNet): the packed-weight cache and the residual / basic
-blocks of their CNN parts on fp16 NC8 buffers.
+"""`TcNet`: the mixin every network with a tensor-core forward (UNet, SwinUNETR, UNETR, DynUNet, SegResNet) inherits.
 
-`TcBlocks` is a mixin for an nn.Module that sets `self._cache = _Cache()`.  The block helpers accept any module with the
-`conv1.conv` / `conv2.conv` / optional `conv3.conv`, `norm1/2/3` and `lrelu` structure of UnetResBlock / UnetBasicBlock
-(dynunet_block.py:25-177; kernel 3, stride 1 or 2, InstanceNorm with or without affine parameters, LeakyReLU).  eps, gamma /
-beta and the slope are read from the block, so the non-affine blocks of the transformer segmenters (eps 1e-5, slope 0.01) call
-exactly the entry points and arguments they did before the affine variants existed."""
+It owns what those networks share:
+  * `forward`: the choice between `_forward_tc` (fp16 channel-blocked "NC8" buffers on Hopper tensor cores) and `_forward_generic`
+    (the generic kernels), through the hooks `_check_input` (both paths), `_use_tc` and `_check_tc_input` (tensor-core path only);
+  * CUDA-graph replay of `_forward_tc`.  One forward is tens to hundreds of short kernel launches; issuing them from Python
+    through ctypes costs more than the kernels themselves once they are fast, so the launch sequence for a given input shape is
+    captured once into a CUDA graph and replayed.  Graphs are keyed by (shape, dtype, device) and invalidated when any parameter
+    changes (`load_state_dict`, `.half()`).  MONAI_B200_GRAPH=0 disables the mechanism;
+  * the packed-weight cache, the channel-padded input stem, and the residual / basic blocks, transposed convolutions and output
+    head of the CNN parts.  The block helpers accept any module with the `conv1.conv` / `conv2.conv` / optional `conv3.conv`,
+    `norm1/2/3` and `lrelu` structure of UnetResBlock / UnetBasicBlock (dynunet_block.py:25-177; kernel 3, stride 1 or 2,
+    InstanceNorm with or without affine parameters, LeakyReLU).  eps, gamma / beta and the slope are read from the block, so the
+    non-affine blocks of the transformer segmenters (eps 1e-5, slope 0.01) call exactly the entry points and arguments they
+    did before the affine variants existed.
+
+A network calls `self._tc_setup()` in its constructor and supplies `_forward_tc` and `_forward_generic`."""
 from __future__ import annotations
 
+import os
 from collections.abc import Sequence
 
 import torch
@@ -16,7 +26,7 @@ import torch.nn as nn
 from ... import _kernels as K
 from ... import _lib as L
 
-__all__ = ["TcBlocks"]
+__all__ = ["TcNet"]
 
 
 class _Cache:
@@ -35,8 +45,65 @@ class _Cache:
         return val
 
 
-class TcBlocks:
+class TcNet:
     _cache: _Cache
+    _tc_ok: bool
+
+    def _tc_setup(self) -> None:
+        self._cache = _Cache()
+        self._graph_enabled = os.environ.get("MONAI_B200_GRAPH", "1") != "0"
+        self._graphs: dict = {}
+
+    # ------------------------------------------------------------------------------------------------- dispatch
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        self._check_input(x)
+        if not self._use_tc(x):
+            return self._forward_generic(x)
+        self._check_tc_input(x)
+        return self._forward_graphed(x) if self._graph_ok() else self._forward_tc(x)
+
+    def _check_input(self, x: torch.Tensor) -> None:
+        """Raises on input neither path accepts."""
+
+    def _use_tc(self, x: torch.Tensor) -> bool:
+        return self._tc_ok and x.is_cuda and x.dtype == torch.float16
+
+    def _check_tc_input(self, x: torch.Tensor) -> None:
+        """Raises, before any launch, on input the tensor-core path does not accept."""
+
+    def _check_levels(self, x: torch.Tensor, levels: int) -> None:
+        """[N, in_channels, D, H, W] with every spatial size divisible by 2^(levels - 1)."""
+        name, div = type(self).__name__, 2 ** (levels - 1)
+        if x.dim() != 5 or x.shape[1] != self.in_channels:
+            raise ValueError(f"{name} expects an [N, {self.in_channels}, D, H, W] input, got {tuple(x.shape)}")
+        if any(int(s) % div for s in x.shape[2:]):
+            raise ValueError(f"{name} with {levels} levels needs spatial sizes divisible by {div}, got {tuple(x.shape[2:])}")
+
+    def _graph_ok(self) -> bool:
+        return self._graph_enabled and not K._Prof.on and not torch.cuda.is_current_stream_capturing()
+
+    def _forward_graphed(self, x_in: torch.Tensor) -> torch.Tensor:
+        sig = tuple((p.data_ptr(), p._version) for p in self.parameters())
+        key = (tuple(x_in.shape), x_in.dtype, x_in.device)
+        ent = self._graphs.get(key)
+        if ent is None or ent["sig"] != sig:
+            static_in = x_in.detach().clone().contiguous()
+            self._forward_tc(static_in)  # eager warm-up: packs weights, sets kernel attributes, fills the plan caches
+            torch.cuda.synchronize(x_in.device)
+            graph = torch.cuda.CUDAGraph()
+            n0 = L.launch_count()
+            # thread_local: other threads (e.g. the NCCL watchdog) may issue CUDA calls while this thread captures
+            with torch.cuda.graph(graph, capture_error_mode="thread_local"):
+                static_out = self._forward_tc(static_in)
+            n_kernels = L.launch_count() - n0
+            if len(self._graphs) >= 4:  # bound the private memory pools kept alive
+                self._graphs.pop(next(iter(self._graphs)))
+            ent = {"sig": sig, "graph": graph, "inp": static_in, "out": static_out, "n_kernels": n_kernels}
+            self._graphs[key] = ent
+        ent["inp"].copy_(x_in)
+        ent["graph"].replay()
+        L.add_replayed_launches(ent["n_kernels"])
+        return ent["out"].clone()
 
     # ----------------------------------------------------------------------------------------------- weight prep
     @staticmethod
@@ -88,6 +155,15 @@ class TcBlocks:
 
     # ------------------------------------------------------------------------------------------------- sub-graphs
     @staticmethod
+    def _pack_input(x_in: torch.Tensor) -> tuple[K.NC8, int]:
+        """The input zero-padded to a multiple of 16 channels (the multi-channel stems run on 16-channel tiles) as an fp16 NC8
+        image; returns (image, padded channel count)."""
+        cp = (x_in.shape[1] + 15) // 16 * 16
+        xz = torch.zeros((x_in.shape[0], cp, *x_in.shape[2:]), device=x_in.device, dtype=torch.float16)
+        K.copy_channels(x_in.to(torch.float16), xz, 0)
+        return K.pack_nc8(xz), cp
+
+    @staticmethod
     def _norm(norm: nn.Module):
         """(eps, gamma, beta) of an InstanceNorm module; gamma / beta are None when it is not affine."""
         if norm.affine:
@@ -115,8 +191,8 @@ class TcBlocks:
     def _basic_block(self, x: K.NC8, cin: int, in_coff: int, blk: nn.Module, key: str, out: K.NC8 | None = None, out_coff: int = 0,
                      x_in_raw: torch.Tensor | None = None, defer_tail: bool = False, cin_pad: int | None = None, stride: int = 1):
         """UnetBasicBlock.forward (dynunet_block.py:165-177) on NC8 buffers: conv1, conv2 with norm1 + lrelu on its operand load,
-        then norm2 + lrelu into `out` (may be a slice of a concat buffer).  With `defer_tail` the last step is NOT applied: (y2,
-        stats2) are returned for the output head."""
+        then norm2 + lrelu into `out` (may be a slice of a concat buffer).  With `defer_tail` the last step is NOT applied: the
+        pieces are returned for `_tail_head` in the form `_res_block` returns them, without a residual."""
         cout = blk.conv1.conv.out_channels
         if x_in_raw is not None:  # single input channel: direct stem kernel on the raw NCDHW window
             y1, st1 = K.conv_cin1_nc8(x_in_raw, blk.conv1.conv.weight, None, 3, 1, 1, want_stats=True)
@@ -124,7 +200,7 @@ class TcBlocks:
             y1, st1 = self._conv1(x, cin, in_coff, blk, key, stride, cin_pad)
         y2, st2 = self._conv2(y1, st1, blk, key)
         if defer_tail:
-            return y2, st2
+            return y2, st2, None, 0, None
         if out is None:
             out = K.NC8(y2.N, cout, y2.sp, y2.buf.device)
         eps2, g2, b2 = self._norm(blk.norm2)
@@ -185,3 +261,22 @@ class TcBlocks:
             K.norm_act_nc8(y2, cout, st2, res=x, res_coff=in_coff, act=L.ACT_LEAKY, slope=slope, out=out, out_coff=out_coff, eps=eps2,
                            gamma=g2, beta=b2)
         return out
+
+    def _up(self, x: K.NC8, cin: int, conv: nn.ConvTranspose3d, key: str, out: K.NC8 | None = None, out_coff: int = 0) -> K.NC8:
+        """ConvTranspose3d k2 s2 as a GEMM whose epilogue scatters to the 2x upsampled voxels (optionally a concat slice)."""
+        y, _ = K.gemm_tc(x, self._wup(conv, key), cin, 8 * conv.out_channels, bias=conv.bias, out=out, out_coff=out_coff, mode=2)
+        return y
+
+    def _up_block(self, x: K.NC8, cin: int, block: nn.Module, cat: K.NC8, key: str, defer_tail: bool = False):
+        """UnetrUpBlock.forward: the transposed convolution writes channels [0, C) of `cat`, whose upper half already holds the
+        skip, then the residual block runs on `cat`."""
+        self._up(x, cin, block.transp_conv.conv, key, out=cat)
+        return self._res_block(cat, cat.C, 0, block.conv_block, key + ".rb", defer_tail=defer_tail)
+
+    def _tail_head(self, tail, block: nn.Module, out_conv: nn.Conv3d, dtype: torch.dtype) -> torch.Tensor:
+        """The 1x1x1 output convolution with the deferred tail of the last block (`defer_tail=True`) -- its norm2, the residual
+        branch if any, and LeakyReLU -- applied on the operand load."""
+        y2, st2, res, res_coff, res_st = tail
+        eps, g, b = self._norm(block.norm2)
+        return K.head_conv_norm_nc8(y2, st2, res, res_coff, res_st, self._slope(block), eps, out_conv.weight, out_conv.bias, out_dtype=dtype,
+                                    gamma=g, beta=b)

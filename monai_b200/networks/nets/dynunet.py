@@ -25,9 +25,8 @@ import torch
 import torch.nn as nn
 
 from ... import _kernels as K
-from .._graph import GraphedForward
 from ..blocks.dynunet_block import UnetBasicBlock, UnetOutBlock, UnetResBlock, UnetUpBlock
-from ._tc_blocks import TcBlocks, _Cache
+from ._tc_blocks import TcNet
 
 __all__ = ["DynUNet", "DynUnet", "Dynunet"]
 
@@ -54,7 +53,7 @@ def _all(v, want: int) -> bool:
     return all(int(i) == want for i in (v if isinstance(v, (list, tuple)) else [v]))
 
 
-class DynUNet(TcBlocks, GraphedForward, nn.Module):
+class DynUNet(TcNet, nn.Module):
     def __init__(
         self,
         spatial_dims: int,
@@ -124,8 +123,7 @@ class DynUNet(TcBlocks, GraphedForward, nn.Module):
 
         self.skip_layers = chain(0, downs, ups, heads)
         self._tc_ok = self._tc_eligible()
-        self._cache = _Cache()
-        self._graph_init()  # the ~100 launches of one tensor-core forward are captured into a CUDA graph per input shape
+        self._tc_setup()
 
     def _tc_eligible(self) -> bool:
         """Whether `_forward_tc` implements this configuration (isotropic 3x3x3 / stride-2 plans, InstanceNorm, LeakyReLU)."""
@@ -168,28 +166,19 @@ class DynUNet(TcBlocks, GraphedForward, nn.Module):
             if module.bias is not None:
                 module.bias = nn.init.constant_(module.bias, 0)
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if not (self._tc_ok and x.is_cuda and x.dtype == torch.float16) or self._dropout_active():
-            return self._forward_generic(x)
+    def _check_input(self, x: torch.Tensor) -> None:
         if self.training and self.deep_supervision:
             raise RuntimeError("monai_b200.DynUNet is inference-only: call .eval() (deep-supervision outputs exist in training mode only)")
-        self._check_tc_input(x)
-        if self._graph_ok():
-            return self._forward_graphed(x, self._forward_tc)
-        return self._forward_tc(x)
+
+    def _use_tc(self, x: torch.Tensor) -> bool:
+        return super()._use_tc(x) and not self._dropout_active()
 
     def _forward_generic(self, x: torch.Tensor) -> torch.Tensor:
-        if self.training and self.deep_supervision:
-            raise RuntimeError("monai_b200.DynUNet is inference-only: call .eval() (deep-supervision outputs exist in training mode only)")
         return self.output_block(self.skip_layers(x))
 
     # ------------------------------------------------------------------------------------------- tensor-core path
     def _check_tc_input(self, x: torch.Tensor) -> None:
-        div = 2 ** (len(self.strides) - 1)
-        if x.dim() != 5 or x.shape[1] != self.in_channels:
-            raise ValueError(f"DynUNet expects an [N, {self.in_channels}, D, H, W] input, got {tuple(x.shape)}")
-        if any(int(s) % div for s in x.shape[2:]):
-            raise ValueError(f"DynUNet with {len(self.strides)} levels needs spatial sizes divisible by {div}, got {tuple(x.shape[2:])}")
+        self._check_levels(x, len(self.strides))
 
     def _forward_tc(self, x_in: torch.Tensor) -> torch.Tensor:
         """DynUNet.forward (dynunet.py:265-274, eval mode) on fp16 NC8 buffers and tensor cores; the output is fp16.
@@ -197,7 +186,6 @@ class DynUNet(TcBlocks, GraphedForward, nn.Module):
         Walks the flat containers.  Level i < last owns one concat buffer of 2 f_i channels: its down block (the input block at
         level 0) writes its normalised output into channels [f_i, 2 f_i) -- the skip, and the input of the next down block --
         and the matching up block's transposed convolution later writes channels [0, f_i)."""
-        self._check_tc_input(x_in)
         with torch.no_grad():
             x_in = x_in.contiguous()
             n, dev, f = x_in.shape[0], x_in.device, self.filters
@@ -208,27 +196,21 @@ class DynUNet(TcBlocks, GraphedForward, nn.Module):
 
             if self.in_channels == 1:   # the raw NCDHW window feeds the single-channel stem kernels
                 block(None, 1, 0, self.input_block, "in", out=cats[0], out_coff=f[0], x_in_raw=x_in)
-            else:                       # several channels: zero-padded to 16 and packed
-                cp = (self.in_channels + 15) // 16 * 16
-                xz = torch.zeros((n, cp, *sp0), device=dev, dtype=torch.float16)
-                K.copy_channels(x_in, xz, 0)
-                block(K.pack_nc8(xz), cp, 0, self.input_block, "in", out=cats[0], out_coff=f[0], cin_pad=cp)
+            else:
+                xp, cp = self._pack_input(x_in)
+                block(xp, cp, 0, self.input_block, "in", out=cats[0], out_coff=f[0], cin_pad=cp)
             for j, down in enumerate(self.downsamples):
                 block(cats[j], f[j], f[j], down, f"d{j}", out=cats[j + 1], out_coff=f[j + 1], stride=2)
             cur = block(cats[nl - 2], f[nl - 2], f[nl - 2], self.bottleneck, "bn", stride=2)
 
             for u, up in enumerate(self.upsamples):
                 lvl = nl - 2 - u
-                tc = up.transp_conv.conv
-                K.gemm_tc(cur, self._wup(tc, f"u{u}.t"), f[lvl + 1], 8 * f[lvl], bias=tc.bias, out=cats[lvl], out_coff=0, mode=2)
+                self._up(cur, f[lvl + 1], up.transp_conv.conv, f"u{u}.t", out=cats[lvl])
                 if lvl > 0:
                     cur = self._basic_block(cats[lvl], 2 * f[lvl], 0, up.conv_block, f"u{u}")
             # the last up block's norm2 + LeakyReLU is applied by the output head on its operand load
-            y2, st2 = self._basic_block(cats[0], 2 * f[0], 0, up.conv_block, f"u{u}", defer_tail=True)
-            eps, g, b = self._norm(up.conv_block.norm2)
-            oc = self.output_block.conv.conv
-            return K.head_conv_norm_nc8(y2, st2, None, 0, None, self._slope(up.conv_block), eps, oc.weight, oc.bias, out_dtype=x_in.dtype,
-                                        gamma=g, beta=b)
+            tail = self._basic_block(cats[0], 2 * f[0], 0, up.conv_block, f"u{u}", defer_tail=True)
+            return self._tail_head(tail, up.conv_block, self.output_block.conv.conv, x_in.dtype)
 
 
 DynUnet = Dynunet = DynUNet

@@ -23,16 +23,15 @@ import torch.nn as nn
 
 from ... import _kernels as K
 from ... import _lib as L
-from .._graph import GraphedForward
 from ..blocks.acti_norm import norm_act_from_modules
 from ..blocks.segresnet_block import ResBlock, get_conv_layer, get_upsample_layer
 from ..layers.factories import get_act_layer, get_norm_layer
-from ._tc_blocks import TcBlocks, _Cache
+from ._tc_blocks import TcNet
 
 __all__ = ["SegResNet"]
 
 
-class SegResNet(TcBlocks, GraphedForward, nn.Module):
+class SegResNet(TcNet, nn.Module):
     def __init__(
         self,
         spatial_dims: int = 3,
@@ -81,8 +80,7 @@ class SegResNet(TcBlocks, GraphedForward, nn.Module):
         if dropout_prob is not None:
             self.dropout = (nn.Dropout, nn.Dropout2d, nn.Dropout3d)[spatial_dims - 1](dropout_prob)
         self._tc_ok = self._tc_eligible()
-        self._cache = _Cache()
-        self._graph_init()  # the ~50-100 launches of one tensor-core forward are captured into a CUDA graph per input shape
+        self._tc_setup()
 
     def _tc_eligible(self) -> bool:
         """Whether `_forward_tc` implements this configuration (3-D, init_filters % 16 == 0, GroupNorm / InstanceNorm, ReLU /
@@ -126,13 +124,8 @@ class SegResNet(TcBlocks, GraphedForward, nn.Module):
             x = self.conv_final[2](norm_act_from_modules(x, self.conv_final[0], self.conv_final[1]))
         return x
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if not (self._tc_ok and x.is_cuda and x.dtype == torch.float16) or self._dropout_active():
-            return self._forward_generic(x)
-        self._check_tc_input(x)
-        if self._graph_ok():
-            return self._forward_graphed(x, self._forward_tc)
-        return self._forward_tc(x)
+    def _use_tc(self, x: torch.Tensor) -> bool:
+        return super()._use_tc(x) and not self._dropout_active()
 
     def _forward_generic(self, x: torch.Tensor) -> torch.Tensor:
         x, down_x = self.encode(x)
@@ -141,16 +134,12 @@ class SegResNet(TcBlocks, GraphedForward, nn.Module):
 
     # ------------------------------------------------------------------------------------------- tensor-core path
     def _check_tc_input(self, x: torch.Tensor) -> None:
-        div = 2 ** (len(self.blocks_down) - 1)
-        if x.dim() != 5 or x.shape[1] != self.in_channels:
-            raise ValueError(f"SegResNet expects an [N, {self.in_channels}, D, H, W] input, got {tuple(x.shape)}")
-        if any(int(s) % div for s in x.shape[2:]):
-            raise ValueError(f"SegResNet with {len(self.blocks_down)} levels needs spatial sizes divisible by {div}, got {tuple(x.shape[2:])}")
+        self._check_levels(x, len(self.blocks_down))
 
     @staticmethod
     def _norm_tc(norm: nn.Module, stats: torch.Tensor, N: int, C: int):
         """(statistics, eps, gamma, beta) for the NC8 norm consumers: a GroupNorm's per-channel sums are folded into group sums."""
-        eps, g, b = TcBlocks._norm(norm)
+        eps, g, b = TcNet._norm(norm)
         groups = norm.num_groups if isinstance(norm, nn.GroupNorm) else C
         return K.group_stats(stats, N, C, groups), eps, g, b
 
@@ -189,19 +178,15 @@ class SegResNet(TcBlocks, GraphedForward, nn.Module):
 
         Every tensor travels with its per-(n, channel) {sum, sumsq}, produced by the epilogue of the launch that wrote it, so each
         GroupNorm costs one tiny `group_stats` launch and is applied on the load of the convolution (or head) that consumes it."""
-        self._check_tc_input(x_in)
         with torch.no_grad():
             x_in = x_in.contiguous()
-            n, dev, f0 = x_in.shape[0], x_in.device, self.init_filters
-            sp0 = tuple(int(s) for s in x_in.shape[2:])
+            n, f0 = x_in.shape[0], self.init_filters
             ci = self.convInit.conv
             if self.in_channels == 1:   # the raw NCDHW window feeds the single-channel stem kernel
                 x, st = K.conv_cin1_nc8(x_in, ci.weight, ci.bias, 3, 1, 1, want_stats=True)
-            else:                       # several channels: zero-padded to 16 and packed
-                cp = (self.in_channels + 15) // 16 * 16
-                xz = torch.zeros((n, cp, *sp0), device=dev, dtype=torch.float16)
-                K.copy_channels(x_in, xz, 0)
-                x, st = K.conv3x3x3_tc(K.pack_nc8(xz), self._w3(ci, "init", cp), cp, f0, bias=ci.bias, want_stats=True)
+            else:
+                xp, cp = self._pack_input(x_in)
+                x, st = K.conv3x3x3_tc(xp, self._w3(ci, "init", cp), cp, f0, bias=ci.bias, want_stats=True)
             # dropout after convInit is the identity in eval mode (forward routes active dropout to the generic path)
 
             down = []

@@ -22,6 +22,7 @@ downsample "merging"/"mergingv2", use_v2 (the residual conv block in front of ev
 from __future__ import annotations
 
 import itertools
+import warnings
 from collections.abc import Sequence
 
 import numpy as np
@@ -30,8 +31,7 @@ import torch.nn as nn
 
 from ... import _kernels as K
 from ... import _lib as L
-from .._graph import GraphedForward
-from ._tc_blocks import TcBlocks, _Cache
+from ._tc_blocks import TcNet
 from ..blocks.acti_norm import norm_act_from_modules
 from ..blocks.convolutions import Convolution, run_conv_module
 
@@ -241,7 +241,7 @@ def window_plan(dims, window_size, shift_size):
     return src.reshape(-1), region, src.shape[0], src.shape[1]
 
 
-class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
+class SwinUNETR(TcNet, nn.Module):
     patch_size: int = 2
 
     def __init__(
@@ -279,7 +279,7 @@ class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
         if spatial_dims != 3:
             raise NotImplementedError("monai_b200 SwinUNETR implements spatial_dims=3")
         # The tensor-core path needs 16-channel multiples (feature_size % 48 == 0) and head_dim 16; every other configuration of the
-        # reference (e.g. its default feature_size = 24: head_dim 8) runs on the generic fp32-faithful kernels (_forward_direct).
+        # reference (e.g. its default feature_size = 24: head_dim 8) runs on the generic fp32-faithful kernels (_forward_generic).
         head_dims = [(feature_size * 2**i) // h for i, h in enumerate(num_heads)]
         if any((feature_size * 2**i) % h for i, h in enumerate(num_heads)) or any(d not in (8, 16, 24, 32, 48, 64) for d in head_dims):
             raise NotImplementedError(f"monai_b200 window attention supports head dimensions 8, 16, 24, 32, 48, 64 (got {head_dims})")
@@ -313,8 +313,7 @@ class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
         self.decoder2 = UnetrUpBlock(2 * fs, fs)
         self.decoder1 = UnetrUpBlock(fs, fs)
         self.out = UnetOutBlock(fs, out_channels)
-        self._cache = _Cache()
-        self._graph_init()  # the ~250 launches of one forward are captured into a CUDA graph per input shape
+        self._tc_setup()
 
     def _check_input_size(self, spatial_shape):
         img_size = np.array(spatial_shape)
@@ -394,7 +393,7 @@ class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
         tmp = K.layernorm_nc8(t, None, None, 1e-5)
         return K.norm_act_nc8(tmp, t.C, None, out=out, out_coff=out_coff)
 
-    def forward(self, x_in: torch.Tensor) -> torch.Tensor:
+    def _check_input(self, x_in: torch.Tensor) -> None:
         if not x_in.is_cuda:
             raise RuntimeError("monai_b200.SwinUNETR runs on CUDA tensors only (there is no CPU fallback)")
         self._check_input_size(x_in.shape[2:])
@@ -402,34 +401,30 @@ class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
             raise ValueError(f"expected {self.in_channels} input channel(s), got {x_in.shape[1]}")
         if x_in.dtype not in (torch.float16, torch.float32):
             raise TypeError(f"SwinUNETR takes float16/float32 inputs, got {x_in.dtype}")
-        if not self._tc_ok or self.fp32_faithful:
-            return self._forward_direct(x_in)
-        if x_in.dtype == torch.float32 and not getattr(self, "_warned_fp32", False):
-            import warnings
 
+    def _use_tc(self, x_in: torch.Tensor) -> bool:
+        return self._tc_ok and not self.fp32_faithful
+
+    def _check_tc_input(self, x_in: torch.Tensor) -> None:
+        if x_in.dtype == torch.float32 and not getattr(self, "_warned_fp32", False):
             # no silent degradation: the tensor-core path stores activations in fp16 (fp32 accumulation everywhere); an fp32
             # input gets fp32 logits of that fp16-storage computation (DESIGN.md section 2: measured ~5e-3 of the output scale)
             warnings.warn("monai_b200.SwinUNETR computes with fp16 activation storage (fp32 accumulation); float32 inputs are converted. "
                           "Expect ~1e-2 relative agreement with an fp32 reference, not 1e-3 (set net.fp32_faithful = True for the fp32 path).")
             self._warned_fp32 = True
-        if self._graph_ok():
-            return self._forward_graphed(x_in, self._forward_impl)
-        return self._forward_impl(x_in)
 
     # --------------------------------------------------------------------------- fp32-faithful generic path
     def _plan_direct(self, dims, ws, ss, dev):
         """window_plan tables on the device + the inverse table (token -> row of the windowed tensor) for window_reverse."""
-        key = ("plan_direct", tuple(dims), tuple(ws), tuple(ss), dev)
-        hit = self._cache.store.get(key)
-        if hit is None:
+        def build():
             src, region, nW, n = window_plan(dims, ws, ss)
             inv = np.full(int(np.prod(dims)), -1, dtype=np.int32)
             rows = np.nonzero(src >= 0)[0]
             inv[src[rows]] = rows.astype(np.int32)
-            hit = (torch.from_numpy(src).to(dev), None if region is None else torch.from_numpy(np.ascontiguousarray(region)).to(dev),
-                   torch.from_numpy(inv).to(dev), nW, n)
-            self._cache.store[key] = hit
-        return hit
+            return (torch.from_numpy(src).to(dev), None if region is None else torch.from_numpy(np.ascontiguousarray(region)).to(dev),
+                    torch.from_numpy(inv).to(dev), nW, n)
+
+        return self._cache.get(("plan_direct", tuple(dims), tuple(ws), tuple(ss), dev), [], build)
 
     def _dense_bias(self, attn: WindowAttention, n: int, key):
         """relative_position_bias_table[relative_position_index[:n, :n]] as float32 [heads, n, n] (swin_unetr.py:514-518)."""
@@ -503,7 +498,7 @@ class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
             t = self._lin(cols, w, None).reshape(N, 2 * C, *(d // 2 for d in dims))
         return t
 
-    def _forward_direct(self, x_in: torch.Tensor) -> torch.Tensor:
+    def _forward_generic(self, x_in: torch.Tensor) -> torch.Tensor:
         """SwinUNETR.forward (swin_unetr.py:316-330) on the generic kernels: activations keep the input's dtype (float32: the
         reference's arithmetic to <= 1e-3), every product accumulates in fp32.  Any feature_size / head dimension of the reference."""
         with torch.no_grad():
@@ -543,7 +538,7 @@ class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
             out = up(dec0, enc0, self.decoder1)
             return self.out.conv(out)
 
-    def _forward_impl(self, x_in: torch.Tensor) -> torch.Tensor:
+    def _forward_tc(self, x_in: torch.Tensor) -> torch.Tensor:
         with torch.no_grad():
             x_in = x_in.contiguous()
             n = x_in.shape[0]
@@ -566,12 +561,9 @@ class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
             if self.in_channels == 1:
                 t0, _ = K.conv_cin1_nc8(x_in, pe.proj.weight, pe.proj.bias, 2, 2, 0)
             else:
-                # several input channels: the volume is repacked once into channel-blocked fp16 with the channels zero-padded to a
-                # multiple of 16, and the stems run on the general tensor-core kernels with zero-padded weights
-                cp = (self.in_channels + 15) // 16 * 16
-                xz = torch.zeros((n, cp, *sp0), device=dev, dtype=torch.float16)
-                K.copy_channels(x_in.to(torch.float16), xz, 0)
-                xp = K.pack_nc8(xz)
+                # several input channels: the volume is repacked once and the stems run on the general tensor-core kernels with
+                # zero-padded weights
+                xp, cp = self._pack_input(x_in)
                 pw = self._cache.get(("pe", cp, pe.proj.weight.device), [pe.proj.weight],
                                      lambda: K.conv_gather_tc_pack_weight(self._pad_cin(pe.proj.weight, cp), 2, 2, 0, False))
                 t0, _ = K.conv_gather_tc(xp, pw, cp, fs, 2, 2, 0, bias=pe.proj.bias)
@@ -592,23 +584,17 @@ class SwinUNETR(TcBlocks, GraphedForward, nn.Module):
             if xp is None:
                 self._res_block(None, 1, 0, self.encoder1.layer, "enc1", out=cat1, out_coff=fs, x_in_raw=x_in)
             else:
-                self._res_block(xp, xp.C, 0, self.encoder1.layer, "enc1", out=cat1, out_coff=fs, cin_pad=xp.C)
+                self._res_block(xp, cp, 0, self.encoder1.layer, "enc1", out=cat1, out_coff=fs, cin_pad=cp)
             self._res_block(h0, fs, 0, self.encoder2.layer, "enc2", out=cat2, out_coff=fs)
             self._res_block(h1, 2 * fs, 0, self.encoder3.layer, "enc3", out=cat3, out_coff=2 * fs)
             self._res_block(h2, 4 * fs, 0, self.encoder4.layer, "enc4", out=cat4, out_coff=4 * fs)
             dec4 = self._res_block(h4, 16 * fs, 0, self.encoder10.layer, "enc10")
 
             # ---- decoders: ConvTranspose k2 s2 scatter into the concat buffer, then the residual block
-            def up(dec_in: K.NC8, cin: int, block: UnetrUpBlock, cat: K.NC8, key: str, defer_tail: bool = False):
-                cout = block.transp_conv.conv.out_channels
-                K.gemm_tc(dec_in, self._wup(block.transp_conv.conv, key), cin, 8 * cout, out=cat, out_coff=0, mode=2)
-                return self._res_block(cat, 2 * cout, 0, block.conv_block, key + ".rb", defer_tail=defer_tail)
-
-            dec3 = up(dec4, 16 * fs, self.decoder5, cat5, "dec5")
-            dec2 = up(dec3, 8 * fs, self.decoder4, cat4, "dec4")
-            dec1 = up(dec2, 4 * fs, self.decoder3, cat3, "dec3")
-            dec0 = up(dec1, 2 * fs, self.decoder2, cat2, "dec2")
+            dec3 = self._up_block(dec4, 16 * fs, self.decoder5, cat5, "dec5")
+            dec2 = self._up_block(dec3, 8 * fs, self.decoder4, cat4, "dec4")
+            dec1 = self._up_block(dec2, 4 * fs, self.decoder3, cat3, "dec3")
+            dec0 = self._up_block(dec1, 2 * fs, self.decoder2, cat2, "dec2")
             # decoder1's norm2 + residual + lrelu is applied by the output head on its operand load (one pass less over 96^3 x 48)
-            y2, st2, res, res_coff, res_st = up(dec0, fs, self.decoder1, cat1, "dec1", defer_tail=True)
-            oc = self.out.conv.conv
-            return K.head_conv_norm_nc8(y2, st2, res, res_coff, res_st, 0.01, 1e-5, oc.weight, oc.bias, out_dtype=x_in.dtype)
+            tail = self._up_block(dec0, fs, self.decoder1, cat1, "dec1", defer_tail=True)
+            return self._tail_head(tail, self.decoder1.conv_block, self.out.conv.conv, x_in.dtype)

@@ -7,7 +7,6 @@ accumulation is fp32.
 """
 from __future__ import annotations
 
-import os
 import warnings
 from collections.abc import Sequence
 
@@ -16,14 +15,14 @@ import torch.nn as nn
 
 from ... import _kernels as K
 from ... import _lib as L
-from .._graph import GraphedForward
 from ..blocks.convolutions import Convolution, ResidualUnit
 from ..layers.simplelayers import SkipConnection
+from ._tc_blocks import TcNet
 
 __all__ = ["UNet", "Unet"]
 
 
-class UNet(GraphedForward, nn.Module):
+class UNet(TcNet, nn.Module):
     def __init__(
         self,
         spatial_dims: int,
@@ -66,8 +65,10 @@ class UNet(GraphedForward, nn.Module):
         self.bias = bias
         self.adn_ordering = adn_ordering
         self.model = self._level(in_channels, out_channels, list(channels), list(strides), True)
-        self._graph_init()
-        self._tc_cache: dict = {}
+        self._tc_setup()
+        # eager: a graph replay copies the input and the output (130 MB per batch of 25 96^3 windows), which costs more than the
+        # ~17 launches of this forward take to issue
+        self._graph_enabled = False
 
     # -- builders (same construction order as the reference so that seeded initialisation matches) -------------
     def _level(self, inc: int, outc: int, channels: list[int], strides: list[int], is_top: bool) -> nn.Module:
@@ -110,11 +111,13 @@ class UNet(GraphedForward, nn.Module):
         return conv
 
     # ------------------------------------------------------------------------------------------ tensor-core path
-    def _tc_eligible(self, x: torch.Tensor) -> bool:
+    def _check_input(self, x: torch.Tensor) -> None:
+        if not x.is_cuda:
+            raise RuntimeError("monai_b200.UNet runs on CUDA tensors only (there is no CPU fallback)")
+
+    def _use_tc(self, x: torch.Tensor) -> bool:
         """fp16 3-D single-channel input, plain conv levels (no residual units), InstanceNorm (non-affine) + PReLU(1) /
         LeakyReLU / ReLU in "NDA" order, 3x3x3 kernels, strides 1 or 2, inner channel counts that are multiples of 16."""
-        if os.environ.get("MONAI_B200_UNET_TC", "1") == "0":
-            return False
         if x.dtype != torch.float16 or self.dimensions != 3 or self.num_res_units != 0 or self.in_channels != 1:
             return False
         if self.kernel_size != 3 or self.up_kernel_size != 3 or self.adn_ordering.upper() != "NDA" or self.dropout not in (0, 0.0, None):
@@ -129,7 +132,7 @@ class UNet(GraphedForward, nn.Module):
             if isinstance(m, nn.PReLU) and m.weight.numel() != 1:
                 return False
             # every conv block on this path applies InstanceNorm (with the module's eps) and then the activation: a block
-            # without a norm (norm=None), with another ordering or with dropout takes the direct path instead
+            # without a norm (norm=None), with another ordering or with dropout takes the generic path instead
             if isinstance(m, Convolution) and m is not self.model[2]:   # model[2]: the top transposed conv (conv only)
                 adn = getattr(m, "adn", None)
                 if adn is None or not isinstance(getattr(adn, "N", None), nn.InstanceNorm3d):
@@ -139,18 +142,10 @@ class UNet(GraphedForward, nn.Module):
                     return False
         return all(isinstance(m, (nn.PReLU, nn.LeakyReLU, nn.ReLU)) for m in self.modules() if type(m).__module__.startswith("torch.nn.modules.activation"))
 
-    def _cached(self, key, params, build):
-        ver = tuple((p.data_ptr(), p._version) for p in params)
-        hit = self._tc_cache.get(key)
-        if hit is None or hit[0] != ver:
-            hit = (ver, build())
-            self._tc_cache[key] = hit
-        return hit[1]
-
     def _act_of(self, conv: Convolution):
         act = getattr(conv.adn, "A", None)
         if isinstance(act, nn.PReLU):
-            return L.ACT_LEAKY, self._cached(("slope", id(act)), [act.weight], lambda: float(act.weight.detach().float().item()))
+            return L.ACT_LEAKY, self._cache.get(("slope", id(act)), [act.weight], lambda: float(act.weight.detach().float().item()))
         if isinstance(act, nn.LeakyReLU):
             return L.ACT_LEAKY, float(act.negative_slope)
         if isinstance(act, nn.ReLU):
@@ -166,7 +161,7 @@ class UNet(GraphedForward, nn.Module):
         if raw is not None:
             y, st = K.conv_cin1_nc8(raw, m.weight, m.bias, k, s, p, want_stats=True)
         else:
-            pw = self._cached(("w", id(m)), [m.weight], lambda: K.conv_gather_tc_pack_weight(m.weight, k, s, p, transposed))
+            pw = self._cache.get(("w", id(m)), [m.weight], lambda: K.conv_gather_tc_pack_weight(m.weight, k, s, p, transposed))
             y, st = K.conv_gather_tc(x, pw, cin, cout, k, s, p, transposed=transposed, output_padding=m.output_padding[0] if transposed else 0,
                                      in_coff=in_coff, bias=m.bias, want_stats=True)
         act, slope = self._act_of(conv)
@@ -196,7 +191,7 @@ class UNet(GraphedForward, nn.Module):
         if top:  # conv only: logits straight to NCDHW
             if upm.out_channels <= 4 and upm.kernel_size[0] == 3 and upm.stride[0] == 2 and upm.padding[0] == 1 and upm.output_padding[0] == 1:
                 return K.convt3s2_head_nc8(cat, c + c_sub, upm.weight, upm.bias, out_dtype=out_dtype)
-            pw = self._cached(("w", id(upm)), [upm.weight], lambda: K.conv_gather_tc_pack_weight(upm.weight, upm.kernel_size[0], upm.stride[0], upm.padding[0], True))
+            pw = self._cache.get(("w", id(upm)), [upm.weight], lambda: K.conv_gather_tc_pack_weight(upm.weight, upm.kernel_size[0], upm.stride[0], upm.padding[0], True))
             y, _ = K.conv_gather_tc(cat, pw, c + c_sub, upm.out_channels, upm.kernel_size[0], upm.stride[0], upm.padding[0], transposed=True,
                                     output_padding=upm.output_padding[0], bias=upm.bias, ncdhw_dtype=out_dtype)
             return y
@@ -206,17 +201,9 @@ class UNet(GraphedForward, nn.Module):
         with torch.no_grad():
             return self._tc_level(self.model, None, 1, x.contiguous(), True, None, 0, x.dtype)
 
-    def _forward_direct(self, x: torch.Tensor) -> torch.Tensor:
+    def _forward_generic(self, x: torch.Tensor) -> torch.Tensor:
         with torch.no_grad():
             return self.model(x.contiguous())
-
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if not x.is_cuda:
-            raise RuntimeError("monai_b200.UNet runs on CUDA tensors only (there is no CPU fallback)")
-        impl = self._forward_tc if self._tc_eligible(x) else self._forward_direct
-        if self._graph_ok() and impl is self._forward_tc:
-            return self._forward_graphed(x, impl)
-        return impl(x)
 
 
 Unet = UNet

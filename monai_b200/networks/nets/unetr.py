@@ -18,10 +18,9 @@ import torch.nn as nn
 
 from ... import _kernels as K
 from ... import _lib as L
-from .._graph import GraphedForward
 from ..blocks.dynunet_block import UnetOutBlock
 from ..blocks.unetr_block import UnetrBasicBlock, UnetrPrUpBlock, UnetrUpBlock
-from ._tc_blocks import TcBlocks, _Cache
+from ._tc_blocks import TcNet
 from .vit import ViT
 
 __all__ = ["UNETR"]
@@ -32,7 +31,7 @@ def _instance_non_affine(norm_name) -> bool:
     return str(name).lower() in ("instance", "instancenorm") and not args.get("affine", False)
 
 
-class UNETR(TcBlocks, GraphedForward, nn.Module):
+class UNETR(TcNet, nn.Module):
     def __init__(self, in_channels: int, out_channels: int, img_size: Sequence[int] | int, feature_size: int = 16, hidden_size: int = 768,
                  mlp_dim: int = 3072, num_heads: int = 12, proj_type: str = "conv", norm_name="instance", conv_block: bool = True,
                  res_block: bool = True, dropout_rate: float = 0.0, spatial_dims: int = 3, qkv_bias: bool = False, save_attn: bool = False) -> None:
@@ -66,23 +65,19 @@ class UNETR(TcBlocks, GraphedForward, nn.Module):
         # configurations the tensor-core forward implements (every other one keeps the generic path)
         self._tc_ok = (spatial_dims == 3 and hidden_size // num_heads == 64 and feature_size % 16 == 0 and mlp_dim % 16 == 0
                        and out_channels <= 16 and _instance_non_affine(norm_name) and conv_block and res_block)
-        self._cache = _Cache()
-        self._graph_init()  # the ~150 launches of one tensor-core forward are captured into a CUDA graph per input shape
+        self._tc_setup()
 
     def proj_feat(self, x: torch.Tensor) -> torch.Tensor:
         """tokens -> feature map.  The reference permutes [N, S, hidden] to [N, hidden, *feat_size]; tokens are already channels-first here."""
         return x.reshape(x.shape[0], self.hidden_size, *self.feat_size)
 
-    def forward(self, x_in: torch.Tensor) -> torch.Tensor:
+    def _check_input(self, x_in: torch.Tensor) -> None:
         if tuple(x_in.shape[2:]) != tuple(f * p for f, p in zip(self.feat_size, self.patch_size)):
             raise ValueError(f"UNETR was built for inputs of size {tuple(f * p for f, p in zip(self.feat_size, self.patch_size))}, got {tuple(x_in.shape[2:])}")
-        if not (self._tc_ok and x_in.is_cuda and x_in.dtype == torch.float16):
-            return self._forward_generic(x_in)
+
+    def _check_tc_input(self, x_in: torch.Tensor) -> None:
         if x_in.shape[1] != self.in_channels:
             raise ValueError(f"expected {self.in_channels} input channel(s), got {x_in.shape[1]}")
-        if self._graph_ok():
-            return self._forward_graphed(x_in, self._forward_tc)
-        return self._forward_tc(x_in)
 
     def _forward_generic(self, x_in: torch.Tensor) -> torch.Tensor:
         x, hidden = self.vit(x_in)
@@ -134,11 +129,6 @@ class UNETR(TcBlocks, GraphedForward, nn.Module):
         nrm = self.vit.norm
         return K.layernorm_nc8(cur, nrm.weight, nrm.bias, nrm.eps), hidden
 
-    def _up(self, x: K.NC8, cin: int, conv: nn.ConvTranspose3d, key: str, out: K.NC8 | None = None, out_coff: int = 0) -> K.NC8:
-        """ConvTranspose3d k2 s2 as a GEMM whose epilogue scatters to the 2x upsampled voxels (optionally a concat slice)."""
-        y, _ = K.gemm_tc(x, self._wup(conv, key), cin, 8 * conv.out_channels, out=out, out_coff=out_coff, mode=2)
-        return y
-
     def _pr_up(self, x: K.NC8, blk: UnetrPrUpBlock, key: str, out: K.NC8, out_coff: int) -> None:
         """UnetrPrUpBlock.forward: the last layer writes the skip slice of the decoder's concat buffer."""
         cout = blk.transp_conv_init.conv.out_channels
@@ -171,24 +161,15 @@ class UNETR(TcBlocks, GraphedForward, nn.Module):
             if self.in_channels == 1:
                 self._res_block(None, 1, 0, self.encoder1.layer, "enc1", out=cat1, out_coff=fs, x_in_raw=x_in)
             else:
-                cp = (self.in_channels + 15) // 16 * 16
-                xz = torch.zeros((n, cp, *sp0), device=dev, dtype=torch.float16)
-                K.copy_channels(x_in, xz, 0)
-                xp = K.pack_nc8(xz)
+                xp, cp = self._pack_input(x_in)
                 self._res_block(xp, cp, 0, self.encoder1.layer, "enc1", out=cat1, out_coff=fs, cin_pad=cp)
             self._pr_up(h3, self.encoder2, "enc2", cat2, 2 * fs)
             self._pr_up(h6, self.encoder3, "enc3", cat3, 4 * fs)
             self._pr_up(h9, self.encoder4, "enc4", cat4, 8 * fs)
 
-            # decoders: ConvTranspose k2 s2 scatter into the concat buffer, then the residual block
-            def up(dec_in: K.NC8, cin: int, block: UnetrUpBlock, cat: K.NC8, key: str, defer_tail: bool = False):
-                self._up(dec_in, cin, block.transp_conv.conv, key, out=cat, out_coff=0)
-                return self._res_block(cat, cat.C, 0, block.conv_block, key + ".rb", defer_tail=defer_tail)
-
-            dec3 = up(tokens, self.hidden_size, self.decoder5, cat4, "dec5")
-            dec2 = up(dec3, 8 * fs, self.decoder4, cat3, "dec4")
-            dec1 = up(dec2, 4 * fs, self.decoder3, cat2, "dec3")
+            dec3 = self._up_block(tokens, self.hidden_size, self.decoder5, cat4, "dec5")
+            dec2 = self._up_block(dec3, 8 * fs, self.decoder4, cat3, "dec4")
+            dec1 = self._up_block(dec2, 4 * fs, self.decoder3, cat2, "dec3")
             # decoder2's norm2 + residual + lrelu is applied by the output head on its operand load
-            y2, st2, res, res_coff, res_st = up(dec1, 2 * fs, self.decoder2, cat1, "dec2", defer_tail=True)
-            oc = self.out.conv.conv
-            return K.head_conv_norm_nc8(y2, st2, res, res_coff, res_st, 0.01, 1e-5, oc.weight, oc.bias, out_dtype=x_in.dtype)
+            tail = self._up_block(dec1, 2 * fs, self.decoder2, cat1, "dec2", defer_tail=True)
+            return self._tail_head(tail, self.decoder2.conv_block, self.out.conv.conv, x_in.dtype)

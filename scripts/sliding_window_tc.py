@@ -1,0 +1,253 @@
+#!/usr/bin/env python
+"""A network with a tensor-core forward as the predictor of a sliding-window inference, on deployed configurations:
+
+  * unetr:               the reference's defaults (ViT-B/16, feature_size 16, 14 classes); a 256^3 fp16 volume, roi 96^3;
+  * dynunet:             the nnU-Net default plan (6 levels, filters 32 ... 320, affine instance norm, 14 classes); a 384^3 fp16
+                         volume, roi 128^3;
+  * segresnet brats:     init_filters 16, 4 input modalities, 3 outputs, GroupNorm(8), blocks (1,2,2,4) / (1,1,1); a
+                         4 x 240 x 240 x 160 fp16 volume, roi 128^3;
+  * segresnet wholebody: init_filters 32, 1 input channel, 105 outputs, GroupNorm(8); a 256^3 fp16 volume, roi 96^3.
+
+    python scripts/sliding_window_tc.py --net unetr|dynunet|segresnet [--workload brats|wholebody|both] [--sw-batch 4]
+                                        [--steps 3] [--warmup 1]
+
+Overlap 0.5, gaussian blending.  Every batch shape (the full batches and the remainder batch) is warmed up first; each timed step
+is bracketed by CUDA events with a 256 MiB L2 flush before it (outside the timed interval), and the spread of the timed steps is
+reported.  A separate profiled step lists device time per kernel.  Finally one forward of sw_batch windows and one of a single
+window are timed on each path: `net(x)` (tensor cores) and `net._forward_generic(x)` (the generic CUDA-core kernels), giving the
+speed-up per window without running a whole volume on CUDA cores.  Prints one JSON line per workload, with the card name and
+power limit read in the same run.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import math
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+
+import torch  # noqa: E402
+
+OVERLAP = 0.5
+
+
+def unetr_flops(net, roi) -> dict:
+    """Multiply-add FLOPs (x2) of one window, from the layer shapes of UNETR.forward (ViT and decoder separately)."""
+    hid, mlp, heads = net.hidden_size, net.mlp_dim, net.num_heads
+    fs, cin = net.feature_size, net.in_channels
+    v = [math.prod(s // 2**k for s in roi) for k in range(5)]   # voxels at 1, 1/2, 1/4, 1/8, 1/16 resolution
+    S = v[4]
+    vit = 2.0 * S * cin * 16**3 * hid
+    vit += net.num_layers * (2.0 * S * hid * 3 * hid + 4.0 * heads * S * S * (hid // heads) + 2.0 * S * hid * hid + 4.0 * S * hid * mlp)
+
+    def res(ci, co, n):      # UnetResBlock: two 3x3x3 convolutions and a 1x1x1 one when the channels change
+        return 2.0 * n * 27 * (ci * co + co * co) + (2.0 * n * ci * co if ci != co else 0.0)
+
+    def up(ci, co, n_in):    # ConvTranspose3d k2 s2
+        return 2.0 * n_in * 8 * ci * co
+
+    dec = res(cin, fs, v[0])
+    dec += up(hid, 2 * fs, v[4]) + up(2 * fs, 2 * fs, v[3]) + res(2 * fs, 2 * fs, v[2]) + up(2 * fs, 2 * fs, v[2]) + res(2 * fs, 2 * fs, v[1])
+    dec += up(hid, 4 * fs, v[4]) + up(4 * fs, 4 * fs, v[3]) + res(4 * fs, 4 * fs, v[2])
+    dec += up(hid, 8 * fs, v[4])
+    dec += up(hid, 8 * fs, v[4]) + res(16 * fs, 8 * fs, v[3])
+    dec += up(8 * fs, 4 * fs, v[3]) + res(8 * fs, 4 * fs, v[2])
+    dec += up(4 * fs, 2 * fs, v[2]) + res(4 * fs, 2 * fs, v[1])
+    dec += up(2 * fs, fs, v[1]) + res(2 * fs, fs, v[0])
+    dec += 2.0 * v[0] * fs * net.out.conv.conv.out_channels
+    return {"vit": vit, "decoder": dec, "total": vit + dec}
+
+
+def dynunet_flops(net, roi) -> dict:
+    """Multiply-add FLOPs (x2) of one window, from the layer shapes of DynUNet.forward (isotropic stride-2 plan)."""
+    f, cin, nl = net.filters, net.in_channels, len(net.filters)
+    v = [math.prod(s // 2**k for s in roi) for k in range(nl)]   # voxels at level k
+    res = net.conv_block.__name__ == "UnetResBlock"
+
+    def block(ci, co, n, skip_conv):   # two 3x3x3 convolutions (+ the 1x1x1 one of a residual block when shape or channels change)
+        return 2.0 * n * 27 * (ci * co + co * co) + (2.0 * n * ci * co if res and skip_conv else 0.0)
+
+    enc = block(cin, f[0], v[0], cin != f[0])
+    for k in range(1, nl):                              # down blocks and the bottleneck (stride 2: output voxels v[k])
+        enc += block(f[k - 1], f[k], v[k], True)
+    dec = 2.0 * v[0] * f[0] * net.out_channels
+    for k in range(nl - 2, -1, -1):                     # up blocks: ConvTranspose3d k2 s2, then a basic block on the concat
+        dec += 2.0 * v[k] * f[k + 1] * f[k] + 2.0 * v[k] * 27 * (2 * f[k] * f[k] + f[k] * f[k])
+    return {"encoder": enc, "decoder": dec, "total": enc + dec}
+
+
+def segresnet_flops(net, roi) -> dict:
+    """Multiply-add FLOPs (x2) of one window, from the layer shapes of SegResNet.forward."""
+    f0, nd = net.init_filters, len(net.blocks_down)
+    v = [math.prod(s // 2**k for s in roi) for k in range(nd)]     # voxels at level k
+    c = [f0 * 2**k for k in range(nd)]                             # channels at level k
+    conv3 = lambda n, ci, co: 2.0 * n * 27 * ci * co               # noqa: E731
+    enc = conv3(v[0], net.in_channels, f0)                         # convInit
+    for k, nb in enumerate(net.blocks_down):
+        if k > 0:
+            enc += conv3(v[k], c[k - 1], c[k])                     # stride-2 pre_conv (output voxels)
+        enc += nb * 2 * conv3(v[k], c[k], c[k])                    # ResBlocks: two 3x3x3 convolutions each
+    dec = 0.0
+    for i, nb in enumerate(net.blocks_up):
+        k = nd - 2 - i                                             # the level the decoder step lands on
+        dec += 2.0 * v[k + 1] * c[k + 1] * c[k]                    # 1x1x1 at the low resolution
+        if net.upsample_mode == "deconv":
+            dec += 2.0 * v[k + 1] * c[k] * c[k] * 8                # ConvTranspose3d k2 s2
+        dec += nb * 2 * conv3(v[k], c[k], c[k])
+    if net.use_conv_final:
+        dec += 2.0 * v[0] * f0 * net.conv_final[2].conv.out_channels
+    return {"encoder": enc, "decoder": dec, "total": enc + dec}
+
+
+def _nets():
+    from monai_b200.networks.nets import UNETR, DynUNet, SegResNet
+
+    return {
+        "unetr": {
+            "unetr_sliding_window": dict(
+                make=lambda: UNETR(in_channels=1, out_channels=14, img_size=(96, 96, 96)), seed=80, cin=1, volume=(256, 256, 256), roi=(96, 96, 96),
+                flops=unetr_flops, desc="UNETR(in=1, out=14, img=96, hidden=768, heads=12, mlp=3072, fs=16)"),
+        },
+        "dynunet": {
+            "dynunet_sliding_window": dict(
+                make=lambda: DynUNet(3, 1, 14, kernel_size=[3] * 6, strides=[1, 2, 2, 2, 2, 2], upsample_kernel_size=[2] * 5), seed=30, cin=1,
+                volume=(384, 384, 384), roi=(128, 128, 128), flops=dynunet_flops,
+                desc="DynUNet(in=1, out=14, k=3x6, strides=[1,2,2,2,2,2], filters=32..320, affine IN)"),
+        },
+        "segresnet": {
+            "segresnet_sliding_window_brats": dict(
+                make=lambda: SegResNet(spatial_dims=3, init_filters=16, in_channels=4, out_channels=3, blocks_down=(1, 2, 2, 4), blocks_up=(1, 1, 1)),
+                seed=30, cin=4, volume=(240, 240, 160), roi=(128, 128, 128), flops=segresnet_flops,
+                desc="SegResNet(init=16, in=4, out=3, GroupNorm(8), blocks (1, 2, 2, 4)/(1, 1, 1), nontrainable)"),
+            "segresnet_sliding_window_wholebody": dict(
+                make=lambda: SegResNet(spatial_dims=3, init_filters=32, in_channels=1, out_channels=105, norm=("GROUP", {"num_groups": 8})),
+                seed=30, cin=1, volume=(256, 256, 256), roi=(96, 96, 96), flops=segresnet_flops,
+                desc="SegResNet(init=32, in=1, out=105, GroupNorm(8), blocks (1, 2, 2, 4)/(1, 1, 1), nontrainable)"),
+        },
+    }
+
+
+def _card() -> dict:
+    out = {"name": torch.cuda.get_device_name(0), "power_limit_w": None, "sm_max_mhz": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", "0"],
+                           capture_output=True, text=True, timeout=30)
+        pl, mx = r.stdout.strip().splitlines()[0].split(", ")
+        out["power_limit_w"], out["sm_max_mhz"] = float(pl), float(mx)
+    except (OSError, ValueError, IndexError, subprocess.TimeoutExpired):
+        pass
+    return out
+
+
+def _windows(volume, roi) -> int:
+    return math.prod(len(range(0, s - r + 1, int(r * (1 - OVERLAP)))) + ((s - r) % int(r * (1 - OVERLAP)) != 0) for s, r in zip(volume, roi))
+
+
+def _timed(fn, x, reps: int) -> float:
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        fn(x)
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def run(metric: str, wl: dict, args, card: dict) -> dict:
+    from weights import fill_state_dict
+
+    from monai_b200 import _kernels as K
+    from monai_b200.inferers import sliding_window_inference
+
+    volume, roi, cin = wl["volume"], wl["roi"], wl["cin"]
+    dev = torch.device("cuda:0")
+    net = wl["make"]()
+    net.load_state_dict(fill_state_dict(net.state_dict(), wl["seed"]))
+    net = net.half().eval().to(dev)
+    assert net._tc_ok
+    vol = torch.randn((1, cin, *volume), generator=torch.Generator().manual_seed(0)).half().to(dev)
+    windows = _windows(volume, roi)
+
+    def step():
+        return sliding_window_inference(vol, roi, args.sw_batch, net, OVERLAP, "gaussian")
+
+    with torch.no_grad():
+        for _ in range(max(1, args.warmup)):   # every batch shape, the remainder batch included
+            step()
+        torch.cuda.synchronize()
+        flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+        times = []
+        for _ in range(args.steps):
+            flush.fill_(1)
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            step()
+            e1.record()
+            torch.cuda.synchronize()
+            times.append(e0.elapsed_time(e1))
+        del flush
+
+        K.profile_start()   # a separate, eager pass: the per-launch events slow the host down
+        step()
+        prof = K.profile_stop()
+        prof_ms = sum(d["ms"] for d in prof.values())
+        top = sorted(prof.items(), key=lambda kv: -kv[1]["ms"])[: args.top]
+
+        per_window = {}
+        for b in sorted({args.sw_batch, 1}):
+            xb = torch.randn((b, cin, *roi), generator=torch.Generator().manual_seed(b)).half().to(dev)
+            net(xb)
+            tc_ms = _timed(net, xb, 5)
+            net._forward_generic(xb)   # loads the generic kernels
+            gen_ms = _timed(net._forward_generic, xb, 1)
+            per_window[f"batch{b}"] = {"tensor_core": round(tc_ms / b, 3), "generic": round(gen_ms / b, 3), "speedup": round(gen_ms / tc_ms, 1)}
+
+    fl = wl["flops"](net, roi)
+    ms = sorted(times)[len(times) // 2]
+    return {
+        "metric": metric,
+        "card": card,
+        "config": {"volume": [cin, *volume], "roi": list(roi), "overlap": OVERLAP, "mode": "gaussian", "sw_batch": args.sw_batch,
+                   "windows": windows, "dtype": "float16", "net": wl["desc"], "l2": "256 MiB flush write between timed steps", "steps": args.steps},
+        "ms_per_step": round(ms, 2), "ms_per_step_min": round(min(times), 2), "ms_per_step_max": round(max(times), 2),
+        "ms_per_step_all": [round(t, 2) for t in times],
+        "voxels_per_s": math.prod(volume) / (ms / 1e3),
+        "gflop_per_window": {k: round(v / 1e9, 2) for k, v in fl.items()},
+        "model_tflops": fl["total"] * windows / (ms / 1e3) / 1e12,
+        "profile_ms_total": round(prof_ms, 2),
+        "top_kernels": [{"name": n, "ms": round(d["ms"], 3), "share": round(d["ms"] / prof_ms, 4), "n": d["n"],
+                         "tflops": round(d["flops"] / (d["ms"] / 1e3) / 1e12, 1) if d["flops"] and d["ms"] else None,
+                         "gbps": round(d["bytes"] / (d["ms"] / 1e3) / 1e9, 1) if d["bytes"] and d["ms"] else None} for n, d in top],
+        "profile_gflop_per_window": round(sum(d["flops"] for d in prof.values()) / windows / 1e9, 2),
+        "per_window_ms": per_window,
+    }
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--net", required=True, choices=["unetr", "dynunet", "segresnet"])
+    ap.add_argument("--workload", default="both", choices=["both", "brats", "wholebody"], help="SegResNet only")
+    ap.add_argument("--sw-batch", type=int, default=4)
+    ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--top", type=int, default=12)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("sliding_window_tc.py measures on a CUDA device; none is available")
+    workloads = _nets()[args.net]
+    if args.net == "segresnet" and args.workload != "both":
+        workloads = {f"segresnet_sliding_window_{args.workload}": workloads[f"segresnet_sliding_window_{args.workload}"]}
+    card = _card()
+    for metric, wl in workloads.items():
+        print(json.dumps(run(metric, wl, args, card)), flush=True)
+
+
+if __name__ == "__main__":
+    main()

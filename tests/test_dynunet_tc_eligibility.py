@@ -1,23 +1,11 @@
 """Which DynUNet configurations the fp16 tensor-core forward implements (`_tc_ok`, decided at construction; CPU only)."""
-import importlib.util
-import os
-
 import pytest
+from dynunet_cases import DYNUNET_CASES as GENERIC
+from tc_cases import TC_CASES
 
 from monai_b200.networks.nets import DynUNet
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _load(name):
-    spec = importlib.util.spec_from_file_location("_" + name, os.path.join(HERE, "golden", name + ".py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-TC = _load("dynunet_tc_cases").DYNUNET_TC_CASES
-GENERIC = _load("dynunet_cases").DYNUNET_CASES
+TC = TC_CASES["dynunet"]
 DEFAULT = TC["A"][0]
 
 

@@ -1,7 +1,6 @@
 """The fp16 tensor-core forward of DynUNet and the affine InstanceNorm of the NC8 kernels (b200_norm_act_affine_nc8,
 b200_conv3x3x3_tc_affine, b200_head_conv_norm_affine_nc8), against torch and against fixtures of the real reference
-(tests/golden/dynunet_tc.npz, configurations in dynunet_tc_cases.py)."""
-import importlib.util
+(tests/golden/dynunet_tc.npz, configurations in tc_cases.py)."""
 import os
 
 import numpy as np
@@ -12,36 +11,15 @@ import torch.nn.functional as F
 from monai_b200 import _kernels as K
 from monai_b200 import _lib as L
 from monai_b200.inferers import sliding_window_inference
+from dynunet_cases import DYNUNET_CASES
 from monai_b200.networks.nets import DynUNet
+from tc_cases import TC_CASES, load_input
 from weights import fill_state_dict
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 TC_KERNELS = {"gemm_tc", "conv3x3x3_tc", "conv3x3x3_tc_affine", "conv_cin1_tc", "conv_gather_tc", "norm_act_nc8", "norm_act_affine_nc8",
               "head_conv_norm_nc8", "head_conv_norm_affine_nc8"}
-
-
-def _load(golden_dir, name):
-    spec = importlib.util.spec_from_file_location("_" + name, os.path.join(golden_dir, name + ".py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-def _cases(golden_dir):
-    mod = _load(golden_dir, "dynunet_tc_cases")
-    return mod.DYNUNET_TC_CASES, mod.make_input
-
-
-def _input(golden_dir, tag, g=None):
-    """The case's fp16 input regenerated from its seed, checked against the sample the fixture keeps of the reference's input."""
-    cases, make_input = _cases(golden_dir)
-    _, shape, _, xseed = cases[tag]
-    g = g if g is not None else np.load(os.path.join(golden_dir, "dynunet_tc.npz"))
-    x = make_input(shape, xseed)
-    s = int(g[f"{tag}.x_stride"])
-    assert np.array_equal(x.numpy()[..., ::s, ::s, ::s], g[f"{tag}.x_sub"]), "regenerated input differs from the reference's"
-    return x.to(DEV)
 
 
 def _build(kw, seed):
@@ -157,12 +135,12 @@ def test_head_conv_norm_affine_vs_torch(Cout):
 # ---------------------------------------------------------------------------------------------------- network
 @pytest.mark.parametrize("tag,half", [("A", False), ("A", True), ("B", False)])
 def test_dynunet_tc_matches_reference_fixture(golden_dir, tag, half):
-    kw, shape, seed, _ = _cases(golden_dir)[0][tag]
+    kw, shape, seed = TC_CASES["dynunet"][tag][:3]
     g = np.load(os.path.join(golden_dir, "dynunet_tc.npz"))
     net = _build(kw, seed)
     if half:
         net = net.half()   # a checkpoint moved to fp16 as a whole takes the same path
-    x = _input(golden_dir, tag, g)
+    x = load_input("dynunet", tag, g).to(DEV)
     y = net(x)
     assert y.dtype == torch.float16 and tuple(y.shape) == (shape[0], kw["out_channels"], *shape[2:])
     y = y.float().cpu().numpy()
@@ -176,10 +154,10 @@ def test_dynunet_tc_matches_reference_fixture(golden_dir, tag, half):
     assert abs(float(y.astype(np.float64).sum()) - ysum) <= 3e-2 * np.abs(ref).max() * y.size   # the whole output, not only the subsample
 
 
-def test_dynunet_dispatch_is_measured(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["A"]
+def test_dynunet_dispatch_is_measured():
+    kw, _, seed = TC_CASES["dynunet"]["A"][:3]
     net = _build(kw, seed)
-    x = _input(golden_dir, "A")[:1]
+    x = load_input("dynunet", "A")[:1].to(DEV)
     K.profile_start()
     net(x)
     fp16 = K.profile_stop()
@@ -193,16 +171,16 @@ def test_dynunet_dispatch_is_measured(golden_dir):
     assert "conv3d_direct" in fp32
 
 
-def _ineligible(golden_dir):
+def _ineligible():
     """Case 1 of the generic fixture (anisotropic plan, filters of 8) and a BatchNorm variant of case A."""
-    kw1, _, seed1 = _load(golden_dir, "dynunet_cases").DYNUNET_CASES[1]
-    kwa, _, seeda, _ = _cases(golden_dir)[0]["A"]
+    kw1, _, seed1 = DYNUNET_CASES[1]
+    kwa, _, seeda = TC_CASES["dynunet"]["A"][:3]
     return [(kw1, seed1, (1, 2, 16, 32, 24)), (dict(kwa, norm_name="batch"), seeda, (1, 1, 32, 32, 32))]
 
 
 @pytest.mark.parametrize("i", [0, 1])
-def test_dynunet_ineligible_configs_take_the_generic_path(golden_dir, i):
-    kw, seed, shape = _ineligible(golden_dir)[i]
+def test_dynunet_ineligible_configs_take_the_generic_path(i):
+    kw, seed, shape = _ineligible()[i]
     net = _build(kw, seed).half()
     assert not net._tc_ok
     x = torch.randn(shape, generator=_gen(50 + i)).half().to(DEV)
@@ -213,10 +191,10 @@ def test_dynunet_ineligible_configs_take_the_generic_path(golden_dir, i):
     assert torch.equal(y, net._forward_generic(x))
 
 
-def test_dynunet_tc_deterministic_graphed_and_follows_new_weights(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["B"]
+def test_dynunet_tc_deterministic_graphed_and_follows_new_weights():
+    kw, _, seed = TC_CASES["dynunet"]["B"][:3]
     net = _build(kw, seed)
-    x = _input(golden_dir, "B")
+    x = load_input("dynunet", "B").to(DEV)
     y1 = net(x)        # captures the graph
     y2 = net(x)        # replays it
     assert torch.equal(y1, y2)
@@ -228,8 +206,8 @@ def test_dynunet_tc_deterministic_graphed_and_follows_new_weights(golden_dir):
     assert torch.equal(y3, fresh._forward_tc(x))
 
 
-def test_dynunet_tc_rejects_bad_shapes(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["A"]
+def test_dynunet_tc_rejects_bad_shapes():
+    kw, _, seed = TC_CASES["dynunet"]["A"][:3]
     net = _build(kw, seed)
     with pytest.raises(ValueError, match="divisible by 32"):
         net(torch.zeros(1, 1, 64, 64, 48, device=DEV, dtype=torch.float16))
@@ -237,8 +215,8 @@ def test_dynunet_tc_rejects_bad_shapes(golden_dir):
         net(torch.zeros(1, 2, 64, 64, 64, device=DEV, dtype=torch.float16))
 
 
-def test_dynunet_tc_sliding_window_vs_generic_fp32(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["A"]
+def test_dynunet_tc_sliding_window_vs_generic_fp32():
+    kw, _, seed = TC_CASES["dynunet"]["A"][:3]
     net = _build(kw, seed)
     vol = torch.randn(1, 1, 96, 80, 64, generator=_gen(95)).half()
     # 4 windows of 64^3 at overlap 0.5: one batch of 3 and a remainder batch of 1

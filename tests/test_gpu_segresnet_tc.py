@@ -1,7 +1,6 @@
 """The fp16 tensor-core forward of SegResNet and its kernels (b200_group_stats, b200_conv3x3x3_tc_affine_add, b200_upsample_add_nc8),
-against torch and against fixtures of the real reference (tests/golden/segresnet_tc.npz, configurations in segresnet_tc_cases.py)."""
+against torch and against fixtures of the real reference (tests/golden/segresnet_tc.npz, configurations in tc_cases.py)."""
 import ctypes as C
-import importlib.util
 import os
 
 import numpy as np
@@ -13,6 +12,7 @@ from monai_b200 import _kernels as K
 from monai_b200 import _lib as L
 from monai_b200.inferers import sliding_window_inference
 from monai_b200.networks.nets import SegResNet
+from tc_cases import TC_CASES, load_input
 from weights import fill_state_dict
 
 pytestmark = pytest.mark.gpu
@@ -20,24 +20,6 @@ DEV = "cuda"
 TC_KERNELS = {"gemm_tc", "conv3x3x3_tc", "conv3x3x3_tc_affine", "conv3x3x3_tc_affine_add", "conv_cin1_tc", "conv_gather_tc", "norm_act_nc8",
               "norm_act_affine_nc8", "head_conv_norm_nc8", "head_conv_norm_affine_nc8", "group_stats", "upsample_add_nc8"}
 GENERIC_ONLY = {"conv3d_direct", "norm_act", "resample_affine", "instnorm_stats"}
-
-
-def _cases(golden_dir):
-    spec = importlib.util.spec_from_file_location("_segresnet_tc_cases", os.path.join(golden_dir, "segresnet_tc_cases.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod.SEGRESNET_TC_CASES, mod.make_input
-
-
-def _input(golden_dir, tag, g=None):
-    """The case's fp16 input regenerated from its seed, checked against the sample the fixture keeps of the reference's input."""
-    cases, make_input = _cases(golden_dir)
-    _, shape, _, xseed = cases[tag]
-    g = g if g is not None else np.load(os.path.join(golden_dir, "segresnet_tc.npz"))
-    x = make_input(shape, xseed)
-    s = int(g[f"{tag}.x_stride"])
-    assert np.array_equal(x.numpy()[..., ::s, ::s, ::s], g[f"{tag}.x_sub"]), "regenerated input differs from the reference's"
-    return x.to(DEV)
 
 
 def _build(kw, seed):
@@ -168,11 +150,11 @@ def test_upsample_add_nc8_vs_torch(scale, sp):
 # ---------------------------------------------------------------------------------------------------- network
 @pytest.mark.parametrize("tag", ["A", "B", "C"])
 def test_segresnet_tc_matches_reference_fixture(golden_dir, tag):
-    kw, shape, seed, _ = _cases(golden_dir)[0][tag]
+    kw, shape, seed = TC_CASES["segresnet"][tag][:3]
     g = np.load(os.path.join(golden_dir, "segresnet_tc.npz"))
     net = _build(kw, seed)
     assert net._tc_ok
-    x = _input(golden_dir, tag, g)
+    x = load_input("segresnet", tag, g).to(DEV)
     y = net(x)
     assert y.dtype == torch.float16 and tuple(y.shape) == (shape[0], kw["out_channels"], *shape[2:])
     y = y.float().cpu().numpy()
@@ -187,10 +169,10 @@ def test_segresnet_tc_matches_reference_fixture(golden_dir, tag):
 
 
 @pytest.mark.parametrize("tag", ["A", "B", "C"])
-def test_segresnet_dispatch_is_measured(golden_dir, tag):
-    kw, _, seed, _ = _cases(golden_dir)[0][tag]
+def test_segresnet_dispatch_is_measured(tag):
+    kw, _, seed = TC_CASES["segresnet"][tag][:3]
     net = _build(kw, seed)
-    x = _input(golden_dir, tag)[:1]
+    x = load_input("segresnet", tag)[:1].to(DEV)
     K.profile_start()
     net(x)
     fp16 = K.profile_stop()
@@ -221,10 +203,10 @@ def test_segresnet_ineligible_configs_take_the_generic_path(kw):
     assert torch.equal(y, net._forward_generic(x))
 
 
-def test_segresnet_tc_deterministic_graphed_and_follows_new_weights(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["A"]
+def test_segresnet_tc_deterministic_graphed_and_follows_new_weights():
+    kw, _, seed = TC_CASES["segresnet"]["A"][:3]
     net = _build(kw, seed)
-    x = _input(golden_dir, "A")
+    x = load_input("segresnet", "A").to(DEV)
     y1 = net(x)        # captures the graph
     y2 = net(x)        # replays it
     assert torch.equal(y1, y2)
@@ -236,17 +218,17 @@ def test_segresnet_tc_deterministic_graphed_and_follows_new_weights(golden_dir):
     assert torch.equal(y3, fresh._forward_tc(x))
 
 
-def test_segresnet_tc_wide_head_graphed_equals_eager(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["B"]
+def test_segresnet_tc_wide_head_graphed_equals_eager():
+    kw, _, seed = TC_CASES["segresnet"]["B"][:3]
     net = _build(kw, seed)
-    x = _input(golden_dir, "B")
+    x = load_input("segresnet", "B").to(DEV)
     y1, y2 = net(x), net(x)
     assert y1.is_contiguous() and torch.equal(y1, y2)
     assert torch.equal(net._forward_tc(x), y1)
 
 
-def test_segresnet_tc_rejects_bad_shapes(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["A"]
+def test_segresnet_tc_rejects_bad_shapes():
+    kw, _, seed = TC_CASES["segresnet"]["A"][:3]
     net = _build(kw, seed)
     with pytest.raises(ValueError, match="divisible by 8"):
         net(torch.zeros(1, 4, 32, 32, 20, device=DEV, dtype=torch.float16))
@@ -254,8 +236,8 @@ def test_segresnet_tc_rejects_bad_shapes(golden_dir):
         net(torch.zeros(1, 2, 32, 32, 32, device=DEV, dtype=torch.float16))
 
 
-def test_segresnet_tc_sliding_window_vs_generic_fp32(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["A"]
+def test_segresnet_tc_sliding_window_vs_generic_fp32():
+    kw, _, seed = TC_CASES["segresnet"]["A"][:3]
     net = _build(kw, seed)
     vol = torch.randn(1, 4, 96, 80, 64, generator=_gen(95)).half()
     # 4 windows of 64^3 at overlap 0.5: one batch of 3 and a remainder batch of 1

@@ -1,6 +1,5 @@
 """The fp16 tensor-core forward of UNETR and its wgmma attention kernel (b200_mhsa_tc), against torch and against fixtures of the
-real reference (tests/golden/unetr_tc.npz, configurations in unetr_tc_cases.py)."""
-import importlib.util
+real reference (tests/golden/unetr_tc.npz, configurations in tc_cases.py)."""
 import math
 import os
 
@@ -11,29 +10,12 @@ import torch
 from monai_b200 import _kernels as K
 from monai_b200.inferers import sliding_window_inference
 from monai_b200.networks.nets import UNETR
+from tc_cases import TC_CASES, load_input
 from weights import fill_state_dict
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 TC_KERNELS = {"gemm_tc", "mhsa_tc", "conv3x3x3_tc", "conv_cin1_tc", "conv_gather_tc", "window_attention_tc", "mlp_fused_tc"}
-
-
-def _cases(golden_dir):
-    spec = importlib.util.spec_from_file_location("_unetr_tc_cases", os.path.join(golden_dir, "unetr_tc_cases.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod.UNETR_TC_CASES, mod.make_input
-
-
-def _input(golden_dir, tag, g=None):
-    """The case's fp16 input regenerated from its seed, checked against the sample the fixture keeps of the reference's input."""
-    cases, make_input = _cases(golden_dir)
-    _, shape, _, xseed = cases[tag]
-    g = g if g is not None else np.load(os.path.join(golden_dir, "unetr_tc.npz"))
-    x = make_input(shape, xseed)
-    s = int(g[f"{tag}.x_stride"])
-    assert np.array_equal(x.numpy()[..., ::s, ::s, ::s], g[f"{tag}.x_sub"]), "regenerated input differs from the reference's"
-    return x.to(DEV)
 
 
 def _build(kw, seed):
@@ -82,12 +64,12 @@ def test_mhsa_tc_refuses_other_head_dims():
 
 @pytest.mark.parametrize("tag", ["A", "B"])
 def test_unetr_tc_matches_reference_fixture(golden_dir, tag):
-    kw, shape, seed, _ = _cases(golden_dir)[0][tag]
+    kw, shape, seed = TC_CASES["unetr"][tag][:3]
     g = np.load(os.path.join(golden_dir, "unetr_tc.npz"))
     net = _build(kw, seed)
     if tag == "A":
         net = net.half()   # a checkpoint moved to fp16 as a whole takes the same path
-    x = _input(golden_dir, tag, g)
+    x = load_input("unetr", tag, g).to(DEV)
     y = net(x)
     assert y.dtype == torch.float16 and tuple(y.shape) == (shape[0], kw["out_channels"], *shape[2:])
     y = y.float().cpu().numpy()
@@ -101,10 +83,10 @@ def test_unetr_tc_matches_reference_fixture(golden_dir, tag):
     assert abs(float(y.astype(np.float64).sum()) - ysum) <= 3e-2 * np.abs(ref).max() * y.size   # the whole output, not only the subsample
 
 
-def test_unetr_dispatch_is_measured(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["A"]
+def test_unetr_dispatch_is_measured():
+    kw, _, seed = TC_CASES["unetr"]["A"][:3]
     net = _build(kw, seed)
-    x = _input(golden_dir, "A")[:1]
+    x = load_input("unetr", "A")[:1].to(DEV)
     K.profile_start()
     net(x)
     fp16 = K.profile_stop()
@@ -118,10 +100,10 @@ def test_unetr_dispatch_is_measured(golden_dir):
     assert "conv3d_direct" in fp32 and "mhsa_cf" in fp32
 
 
-def test_unetr_tc_deterministic_graphed_and_follows_new_weights(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["B"]
+def test_unetr_tc_deterministic_graphed_and_follows_new_weights():
+    kw, _, seed = TC_CASES["unetr"]["B"][:3]
     net = _build(kw, seed)
-    x = _input(golden_dir, "B")
+    x = load_input("unetr", "B").to(DEV)
     y1 = net(x)        # captures the graph
     y2 = net(x)        # replays it
     assert torch.equal(y1, y2)
@@ -133,8 +115,8 @@ def test_unetr_tc_deterministic_graphed_and_follows_new_weights(golden_dir):
     assert torch.equal(y3, fresh._forward_tc(x))
 
 
-def test_unetr_tc_sliding_window_vs_generic_fp32(golden_dir):
-    kw, _, seed, _ = _cases(golden_dir)[0]["A"]
+def test_unetr_tc_sliding_window_vs_generic_fp32():
+    kw, _, seed = TC_CASES["unetr"]["A"][:3]
     net = _build(kw, seed)
     vol = torch.randn(1, 1, 128, 112, 96, generator=torch.Generator().manual_seed(95)).half()
     # 4 windows of 96^3 at overlap 0.5: one batch of 3 and a remainder batch of 1

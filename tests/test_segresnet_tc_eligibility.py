@@ -1,22 +1,10 @@
 """Which SegResNet configurations the fp16 tensor-core forward implements (`_tc_ok`, decided at construction; CPU only)."""
-import importlib.util
-import os
-
 import pytest
+from tc_cases import TC_CASES
 
 from monai_b200.networks.nets import SegResNet
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _load(name):
-    spec = importlib.util.spec_from_file_location("_" + name, os.path.join(HERE, "golden", name + ".py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-TC = _load("segresnet_tc_cases").SEGRESNET_TC_CASES
+TC = TC_CASES["segresnet"]
 BRATS = TC["A"][0]
 
 
