@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 2
+#define B200_ABI_VERSION 3
 
 /* ---- library ---------------------------------------------------------------------------------------- */
 int b200_abi_version(void);
@@ -200,6 +200,19 @@ typedef struct b200_conv_tc_desc {
   void* res_y;
   int res_ctot, res_coff;
   float* res_stats;
+  /* AFFINE operand normalisation (InstanceNorm3d(affine=True), dynunet_block.py:114-177; needs in_stats): the kernel feeds
+   * act((x - mean) * rstd * in_gamma + in_beta), the fp16 values b200_norm_act_nc8 with gamma / beta would have stored.
+   * float32 device [Cin]; either may be NULL (1 / 0). */
+  const float* in_gamma;
+  const float* in_beta;
+  /* Identity branch of a pre-activation residual block added in the epilogue (add == NULL = off; needs in_stats, exclusive with
+   * res_w; SegResNet's ResBlock, segresnet_block.py:83-94: x + conv2(act(norm2(y1)))): y = conv(act(norm(x))) + add.  add =
+   * channels [add_coff, add_coff + Cout) of an NC8 fp16 buffer with add_ctot channels and the output's (N, D, H, W), 16-byte
+   * aligned; the sum is formed in fp32 before the single fp16 rounding, and stats are those of the sum.  add may not overlap y
+   * except as the same slice.  The add may run shallower tiles, whose statistics scratch can be larger: the workspace query
+   * sizes it from the same descriptor. */
+  const void* add;
+  int add_ctot, add_coff;
 } b200_conv_tc_desc;
 
 /* 3x3x3, stride 1, zero padding 1 implicit-GEMM convolution on wgmma tensor cores: halo tile staged once
@@ -208,26 +221,13 @@ typedef struct b200_conv_tc_desc {
  * extra pass.  The sums are DETERMINISTIC (bit-identical run to run): the epilogue warps write partial rows into
  * `workspace` (device scratch of b200_conv3x3x3_tc_workspace_bytes(desc) bytes, required when stats != NULL; no
  * initialisation needed) and a finishing pass adds them in a fixed order -- no floating-point atomics anywhere.
- * replaces the Conv3d inside UnetResBlock (monai/networks/blocks/dynunet_block.py:25-111) for SwinUNETR / DynUNet blocks. */
+ * replaces the Conv3d inside UnetResBlock (monai/networks/blocks/dynunet_block.py:25-111) for SwinUNETR / DynUNet blocks.
+ * The descriptor selects the form: plain, with the folded residual (res_w), or with the operand normalisation (in_stats),
+ * optionally affine (in_gamma / in_beta) and with the epilogue add (add).  The workspace query validates the descriptor as
+ * the launch does and returns -1 for one the launch would reject. */
 long long b200_conv3x3x3_tc_workspace_bytes(const b200_conv_tc_desc* desc);
 int b200_conv3x3x3_tc(const b200_conv_tc_desc* desc, const void* x, const void* packed_w, const float* bias,
                       void* y, float* stats, void* workspace, void* stream);
-/* The same with an AFFINE operand normalisation (InstanceNorm3d(affine=True), dynunet_block.py:114-177): desc->in_stats is
- * required and the kernel feeds act((x - mean) * rstd * in_gamma + in_beta), the fp16 values b200_norm_act_affine_nc8 would
- * have stored.  in_gamma / in_beta: float32 device [Cin] (either may be NULL: 1 / 0).  Workspace as for b200_conv3x3x3_tc. */
-int b200_conv3x3x3_tc_affine(const b200_conv_tc_desc* desc, const float* in_gamma, const float* in_beta, const void* x,
-                             const void* packed_w, const float* bias, void* y, float* stats, void* workspace, void* stream);
-
-/* The same with the identity branch of a pre-activation residual block added in the epilogue (SegResNet's ResBlock,
- * segresnet_block.py:83-94: x + conv2(act(norm2(y1)))): y = conv(act(norm(x))) + add.  add = channels [add_coff, add_coff + Cout)
- * of an NC8 fp16 buffer with add_ctot channels and the output's (N, D, H, W); the sum is formed in fp32 before the single fp16
- * rounding, and stats are those of the sum.  desc->in_stats is required and desc->res_w must be NULL; in_gamma / in_beta as for
- * b200_conv3x3x3_tc_affine.  add may not overlap y except as the same slice.  workspace: b200_conv3x3x3_tc_affine_add_workspace_bytes(desc)
- * bytes (the add may run shallower tiles than b200_conv3x3x3_tc, so its statistics scratch can be larger). */
-long long b200_conv3x3x3_tc_affine_add_workspace_bytes(const b200_conv_tc_desc* desc);
-int b200_conv3x3x3_tc_affine_add(const b200_conv_tc_desc* desc, const float* in_gamma, const float* in_beta, const void* x,
-                                 const void* packed_w, const float* bias, const void* add, int add_ctot, int add_coff, void* y,
-                                 float* stats, void* workspace, void* stream);
 
 typedef struct b200_conv_gather_desc {
   int N, Cin, Cout;         /* Cin % 16 == 0; Cout arbitrary for NCDHW output, % 8 == 0 for NC8 output */
@@ -394,35 +394,27 @@ int b200_head_conv_nc8(const void* x, int N, int C, long long S, const float* we
 /* Output head fused with the tail of the last residual block: y = W * lrelu(instnorm(x) + instnorm?(res)) + b
  * (UnetResBlock.forward norm2 + residual + lrelu, dynunet_block.py:97-111, then UnetOutBlock :247-267).  x is a whole NC8
  * tensor of C channels with its (sum, sum of squares) statistics [N*C*2]; res is a channel slice of an NC8 buffer, normalised
- * with res_stats when given (the block's conv3 branch) or added as is. */
+ * with res_stats when given (the block's conv3 branch) or added as is.  gamma / beta: the affine parameters of x's InstanceNorm
+ * (DynUNet's last up block, dynunet_block.py:165-177), float32 device [C]; either may be NULL (1 / 0). */
 int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
                             int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
-                            const float* bias, int Cout, void* y, int out_dtype, void* stream);
-/* The same with an affine InstanceNorm of x (DynUNet's last up block, dynunet_block.py:165-177): gamma / beta float32 device [C]
- * (either may be NULL: 1 / 0). */
-int b200_head_conv_norm_affine_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
-                                   int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
-                                   const float* bias, int Cout, void* y, int out_dtype, const float* gamma, const float* beta,
-                                   void* stream);
+                            const float* bias, int Cout, void* y, int out_dtype, const float* gamma, const float* beta,
+                            void* stream);
 
-/* NC8 variant of b200_norm_act: y = act(instnorm(x) [+ instnorm?(res)]); act: 0 none, 1 leaky-relu(slope), 3 relu.
- * x / res / y are channel slices [coff, coff+C) of NC8 buffers with ctot channels. */
+/* NC8 variant of b200_norm_act: y = act(instnorm(x) * gamma + beta [+ instnorm?(res) * res_gamma + res_beta]); act: 0 none,
+ * 1 leaky-relu(slope), 3 relu.  x / res / y are channel slices [coff, coff+C) of NC8 buffers with ctot channels.  The affine
+ * parameters (UnetResBlock norm2 and norm3 with affine=True, dynunet_block.py:97-111) are float32 device [C] or NULL (1 / 0);
+ * gamma / beta need stats, res_gamma / res_beta need res_stats. */
 int b200_norm_act_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats, float eps,
                       const void* res, int res_ctot, int res_coff, const float* res_stats, int act, float slope,
-                      void* y, int y_ctot, int y_coff, void* stream);
-/* The same with affine InstanceNorms: y = act(instnorm(x) * gamma + beta [+ instnorm(res) * res_gamma + res_beta]) (UnetResBlock
- * norm2 and norm3 with affine=True, dynunet_block.py:97-111).  Each parameter is float32 device [C] or NULL (1 / 0); gamma / beta
- * need stats, res_gamma / res_beta need res_stats.  With all four NULL the output is bit-identical to b200_norm_act_nc8. */
-int b200_norm_act_affine_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats, float eps,
-                             const void* res, int res_ctot, int res_coff, const float* res_stats, int act, float slope,
-                             void* y, int y_ctot, int y_coff, const float* gamma, const float* beta, const float* res_gamma,
-                             const float* res_beta, void* stream);
+                      void* y, int y_ctot, int y_coff, const float* gamma, const float* beta, const float* res_gamma,
+                      const float* res_beta, void* stream);
 
 /* GroupNorm statistics from per-channel ones (nn.GroupNorm, SegResNet's default norm): stats = {sum, sumsq} per (n, channel)
  * [N][C][2] as written by the `stats` outputs of these entry points; for channel c of group g (cpg = C / groups channels each)
  * out[n][c] = {sum over c' in g of sum[n][c'] / cpg, likewise sumsq}, added in fp64 in channel order.  Fed these folded
- * statistics, every NC8 consumer (b200_norm_act(_affine)_nc8, the operand normalisation of b200_conv3x3x3_tc(_affine),
- * b200_head_conv_norm(_affine)_nc8) normalises with the group's mean and variance, fused or not with the same bits.  out may not
+ * statistics, every NC8 consumer (b200_norm_act_nc8, the operand normalisation of b200_conv3x3x3_tc, b200_head_conv_norm_nc8)
+ * normalises with the group's mean and variance, fused or not with the same bits.  out may not
  * alias stats.  With groups == C the output equals the input (callers skip the launch). */
 int b200_group_stats(const float* stats, int N, int C, int groups, float* out, void* stream);
 

@@ -41,24 +41,25 @@ def profile_stop(by_shape: bool = False) -> dict:
     return out
 
 
-def _call(name: str, *args, flops: float = 0.0, nbytes: float = 0.0) -> None:
+def _call(name: str, *args, flops: float = 0.0, nbytes: float = 0.0, label: str | None = None) -> None:
     """Launch one C-ABI entry point (b200_<name>) and raise on a non-zero status.  The launch runs with the device of the
-    stream handle among `args` current (see _lib.stream_ptr), so tensors on a non-current GPU work."""
+    stream handle among `args` current (see _lib.stream_ptr), so tensors on a non-current GPU work.  `label` names the launch
+    in the profile (default: `name`), so that the forms of one entry point are timed apart."""
     fn = getattr(L.load(), "b200_" + name)
     dev = L.take_stream_device()   # the device whose stream handle is among `args`
     if dev is not None and dev.index is not None and dev.index != torch.cuda.current_device():
         with torch.cuda.device(dev):   # kernels, tensor maps and events belong to the tensors' device, not to the current one
-            return _call_on(fn, name, args, flops, nbytes)
-    return _call_on(fn, name, args, flops, nbytes)
+            return _call_on(fn, name, args, flops, nbytes, label or name)
+    return _call_on(fn, name, args, flops, nbytes, label or name)
 
 
-def _call_on(fn, name, args, flops, nbytes) -> None:
+def _call_on(fn, name, args, flops, nbytes, label) -> None:
     if _Prof.on:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         rc = fn(*args)
         e1.record()
-        _Prof.events.append((name, e0, e1, flops, nbytes))
+        _Prof.events.append((label, e0, e1, flops, nbytes))
     else:
         rc = fn(*args)
     L.check(rc, name)
@@ -557,13 +558,14 @@ def conv3x3x3_tc(
     `res_w` = gemm_tc_pack_weight image of a 1x1x1 convolution [Cout, Cin] of the SAME input: it is computed by the same launch
     and the call returns (out, stats, res_out, res_stats) instead of (out, stats).
     `add` = (NC8 tensor, channel offset): channels [coff, coff + Cout) of it, with the output's shape, are added to the result in
-    fp32 before its fp16 store, and the statistics are those of the sum (b200_conv3x3x3_tc_affine_add); it needs `in_norm`."""
+    fp32 before its fp16 store, and the statistics are those of the sum; it needs `in_norm`."""
     if out is None:
         out = NC8(x.N, Cout, x.sp, x.buf.device)
     dev = x.buf.device
     stats = torch.empty((x.N * Cout, 2), device=dev, dtype=torch.float32) if want_stats else None
     b32 = _f32c(bias)
-    d = L.ConvTcDesc(x.N, Cin, Cout, x.sp[0], x.sp[1], x.sp[2], x.C, in_coff, out.C, out_coff, None, 0.0, 0, 0.0, None, None, 0, 0, None)
+    d = L.ConvTcDesc(N=x.N, Cin=Cin, Cout=Cout, D=x.sp[0], H=x.sp[1], W=x.sp[2], in_ctot=x.C, in_coff=in_coff, out_ctot=out.C,
+                     out_coff=out_coff)
     res_out = res_stats = None
     if res_w is not None:
         if in_norm is not None or Cout > 128:
@@ -576,11 +578,11 @@ def conv3x3x3_tc(
         if st.dtype != torch.float32 or st.numel() != x.N * Cin * 2 or not st.is_contiguous() or st.device != dev:
             raise ValueError("conv3x3x3_tc: in_norm statistics must be a contiguous float32 [N*Cin, 2] tensor on the input's device")
         d.in_stats, d.in_eps, d.in_act, d.in_slope = L.ptr(st), float(eps), int(act), float(slope)
-    query = L.load().b200_conv3x3x3_tc_affine_add_workspace_bytes if add is not None else L.load().b200_conv3x3x3_tc_workspace_bytes
-    ws = _ws(query(C.byref(d)), dev) if want_stats else None
-    affine = in_affine is not None and any(t is not None for t in in_affine)
-    if affine and in_norm is None:
+    g32, be32 = (_f32c(t) for t in (in_affine or (None, None)))
+    if (g32 is not None or be32 is not None) and in_norm is None:
         raise ValueError("conv3x3x3_tc: in_affine needs in_norm")
+    d.in_gamma, d.in_beta = L.ptr(g32), L.ptr(be32)
+    label = "conv3x3x3_tc_affine" if g32 is not None or be32 is not None else "conv3x3x3_tc"
     if add is not None:
         a, a_coff = add
         if in_norm is None or res_w is not None:
@@ -588,16 +590,12 @@ def conv3x3x3_tc(
         if a.N != x.N or a.sp != x.sp or a_coff % 8 or a_coff + Cout > a.C:
             raise ValueError(f"conv3x3x3_tc: add must be a channel slice of an NC8 tensor of the output's shape, got {a.C} channels at "
                              f"{a.sp} (offset {a_coff}) for {Cout} channels at {x.sp}")
-        g, b = (in_affine or (None, None))
-        name, extra = "conv3x3x3_tc_affine_add", (L.ptr(_f32c(g)), L.ptr(_f32c(b)))
-        tail = (L.ptr(a.buf), a.C, int(a_coff))
-    elif affine:
-        name, extra, tail = "conv3x3x3_tc_affine", (L.ptr(_f32c(in_affine[0])), L.ptr(_f32c(in_affine[1]))), ()
-    else:
-        name, extra, tail = "conv3x3x3_tc", (), ()
-    _call(name, C.byref(d), *extra, L.ptr(x.buf), L.ptr(packed_w), L.ptr(b32), *tail, L.ptr(out.buf), L.ptr(stats), L.ptr(ws), L.stream_ptr(dev),
+        d.add, d.add_ctot, d.add_coff = L.ptr(a.buf), a.C, int(a_coff)
+        label = "conv3x3x3_tc_affine_add"
+    ws = _ws(L.load().b200_conv3x3x3_tc_workspace_bytes(C.byref(d)), dev) if want_stats else None
+    _call("conv3x3x3_tc", C.byref(d), L.ptr(x.buf), L.ptr(packed_w), L.ptr(b32), L.ptr(out.buf), L.ptr(stats), L.ptr(ws), L.stream_ptr(dev),
           flops=2.0 * x.N * x.S * Cin * Cout * (28 if res_w is not None else 27),
-          nbytes=float(x.N * x.S * (Cin + Cout * (2 if res_w is not None or add is not None else 1)) * 2) + _nb(packed_w))
+          nbytes=float(x.N * x.S * (Cin + Cout * (2 if res_w is not None or add is not None else 1)) * 2) + _nb(packed_w), label=label)
     if res_w is not None:
         return out, stats, res_out, res_stats
     return out, stats
@@ -628,13 +626,11 @@ def norm_act_nc8(
     parameters of x's (res's) InstanceNorm."""
     if out is None:
         out = NC8(x.N, C_, x.sp, x.buf.device)
-    affine = (gamma, beta, res_gamma, res_beta)
-    name, extra = "norm_act_nc8", ()
-    if any(t is not None for t in affine):
-        name, extra = "norm_act_affine_nc8", tuple(L.ptr(_f32c(t)) for t in affine)
-    _call(name, L.ptr(x.buf), x.C, x_coff, x.N, C_, x.S, L.ptr(stats), eps, L.ptr(res.buf) if res is not None else None,
-          res.C if res is not None else 0, res_coff, L.ptr(res_stats), act, float(slope), L.ptr(out.buf), out.C, out_coff, *extra,
-          L.stream_ptr(x.buf.device))
+    affine = [_f32c(t) for t in (gamma, beta, res_gamma, res_beta)]
+    _call("norm_act_nc8", L.ptr(x.buf), x.C, x_coff, x.N, C_, x.S, L.ptr(stats), eps, L.ptr(res.buf) if res is not None else None,
+          res.C if res is not None else 0, res_coff, L.ptr(res_stats), act, float(slope), L.ptr(out.buf), out.C, out_coff,
+          *map(L.ptr, affine), L.stream_ptr(x.buf.device),
+          label="norm_act_affine_nc8" if any(t is not None for t in affine) else "norm_act_nc8")
     return out
 
 
@@ -885,13 +881,13 @@ def head_conv_norm_nc8(x: NC8, stats: torch.Tensor, res: NC8 | None, res_coff: i
     Cout = weight.shape[0]
     w32 = _f32c(weight)
     b32 = _f32c(bias)
+    g32, be32 = _f32c(gamma), _f32c(beta)
     y = torch.empty((x.N, Cout, *x.sp), device=x.buf.device, dtype=out_dtype)
-    name, extra = "head_conv_norm_nc8", ()
-    if gamma is not None or beta is not None:
-        name, extra = "head_conv_norm_affine_nc8", (L.ptr(_f32c(gamma)), L.ptr(_f32c(beta)))
-    _call(name, L.ptr(x.buf), x.N, x.C, x.S, L.ptr(stats), float(eps), L.ptr(res.buf) if res is not None else None,
-          res.C if res is not None else 0, res_coff, L.ptr(res_stats), float(slope), L.ptr(w32), L.ptr(b32), Cout, L.ptr(y), L.dt(y), *extra,
-          L.stream_ptr(x.buf.device), nbytes=float(x.N * x.S * (x.C * (4 if res is not None else 2) + Cout * y.element_size())))
+    _call("head_conv_norm_nc8", L.ptr(x.buf), x.N, x.C, x.S, L.ptr(stats), float(eps), L.ptr(res.buf) if res is not None else None,
+          res.C if res is not None else 0, res_coff, L.ptr(res_stats), float(slope), L.ptr(w32), L.ptr(b32), Cout, L.ptr(y), L.dt(y),
+          L.ptr(g32), L.ptr(be32), L.stream_ptr(x.buf.device),
+          nbytes=float(x.N * x.S * (x.C * (4 if res is not None else 2) + Cout * y.element_size())),
+          label="head_conv_norm_affine_nc8" if gamma is not None or beta is not None else "head_conv_norm_nc8")
     return y
 
 

@@ -14,7 +14,7 @@ import torch
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = _HERE / "lib" / "libmonai_b200.so"
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 DT_F32, DT_F16 = 0, 1
 _DT = {torch.float32: DT_F32, torch.float16: DT_F16}
 
@@ -52,6 +52,7 @@ class ConvTcDesc(C.Structure):
         ("in_ctot", i32), ("in_coff", i32), ("out_ctot", i32), ("out_coff", i32),
         ("in_stats", vp), ("in_eps", f32), ("in_act", i32), ("in_slope", f32),
         ("res_w", vp), ("res_y", vp), ("res_ctot", i32), ("res_coff", i32), ("res_stats", vp),
+        ("in_gamma", vp), ("in_beta", vp), ("add", vp), ("add_ctot", i32), ("add_coff", i32),
     ]
 
 
@@ -96,9 +97,6 @@ SIGNATURES = {
     "b200_conv3x3x3_tc_pack_weight": (i32, [vp, i32, i32, vp, vp]),
     "b200_conv3x3x3_tc_workspace_bytes": (i64, [C.POINTER(ConvTcDesc)]),
     "b200_conv3x3x3_tc": (i32, [C.POINTER(ConvTcDesc), vp, vp, vp, vp, vp, vp, vp]),
-    "b200_conv3x3x3_tc_affine": (i32, [C.POINTER(ConvTcDesc), vp, vp, vp, vp, vp, vp, vp, vp, vp]),
-    "b200_conv3x3x3_tc_affine_add_workspace_bytes": (i64, [C.POINTER(ConvTcDesc)]),
-    "b200_conv3x3x3_tc_affine_add": (i32, [C.POINTER(ConvTcDesc), vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]),
     "b200_conv_gather_tc_weight_bytes": (i64, [C.POINTER(ConvGatherDesc)]),
     "b200_conv_gather_tc_pack_weight": (i32, [C.POINTER(ConvGatherDesc), vp, vp, vp]),
     "b200_conv_gather_tc_workspace_bytes": (i64, [C.POINTER(ConvGatherDesc)]),
@@ -129,10 +127,8 @@ SIGNATURES = {
     "b200_patch_finalize": (i32, [vp, vp, i32, i64, vp]),
     "b200_channel_post": (i32, [vp, i32, i32, i64, i32, f32, i32, vp, i32, vp]),
     "b200_head_conv_nc8": (i32, [vp, i32, i32, i64, vp, vp, i32, vp, i32, vp]),
-    "b200_head_conv_norm_nc8": (i32, [vp, i32, i32, i64, vp, f32, vp, i32, i32, vp, f32, vp, vp, i32, vp, i32, vp]),
-    "b200_head_conv_norm_affine_nc8": (i32, [vp, i32, i32, i64, vp, f32, vp, i32, i32, vp, f32, vp, vp, i32, vp, i32, vp, vp, vp]),
-    "b200_norm_act_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, i32, i32, vp, i32, f32, vp, i32, i32, vp]),
-    "b200_norm_act_affine_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, i32, i32, vp, i32, f32, vp, i32, i32, vp, vp, vp, vp, vp]),
+    "b200_head_conv_norm_nc8": (i32, [vp, i32, i32, i64, vp, f32, vp, i32, i32, vp, f32, vp, vp, i32, vp, i32, vp, vp, vp]),
+    "b200_norm_act_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, i32, i32, vp, i32, f32, vp, i32, i32, vp, vp, vp, vp, vp]),
     "b200_norm_act_cin1res_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, vp, vp, i32, f32, vp, i32, i32, vp]),
     "b200_group_stats": (i32, [vp, i32, i32, i32, vp, vp]),
     "b200_upsample_add_nc8_workspace_bytes": (i64, [i32] * 6),

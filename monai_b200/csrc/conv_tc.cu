@@ -145,10 +145,9 @@ struct ConvTcParams {
   ConvEpiP r;             // RES: output stage of the folded 1x1x1 residual convolution
   const __half* res_w;     // RES: packed 1x1x1 weights (gemm_tc image: [nt][k16][khalf][NT/8][8][8])
 };
-// NORM: affine parameters of the operand's InstanceNorm, float32 [Cin] (NULL = 1 / 0); a kernel argument of its own, so that
-// ConvTcParams (and the code generated around it) is what it was before the affine variant existed
+// NORM: in_gamma / in_beta of the descriptor, and ADD: its add / add_ctot / add_coff, copied into kernel arguments of their own: read
+// from ConvTcParams::d instead, they change the register assignment and scheduling of some instantiations
 struct ConvTcAffine { const float* gamma; const float* beta; };
-// ADD: the tensor added in the epilogue (conv_epi.cuh), channel slice [coff, coff + Cout) of an NC8 buffer with ctot channels
 struct ConvTcAdd { const __half* x; int ctot, coff; };
 
 // Persistent, warp-specialised (384 threads, one CTA per SM): warp 0 = TMA producer, warps 4-7 and 8-11 = two consumer
@@ -531,9 +530,6 @@ struct ConvTcGeom {
 // what a launch needs beyond the operands: mode 0 = run, mode 1 = only report the statistics workspace size
 struct ConvTcCall {
   const void* x; const void* w; const float* bias; void* y; float* stats; void* ws; cudaStream_t st; long long ws_bytes; int query;
-  const float* in_gamma; const float* in_beta;   // NORM: affine parameters of the operand normalisation (NULL = non-affine)
-  ConvTcAdd add;                                 // ADD: tensor added in the epilogue
-  bool has_add;                                  // ADD selected (also in a workspace query, where add.x is not given)
 };
 
 template <int NT, int BD, bool NORM, bool RES = false, bool ADD = false>
@@ -571,16 +567,17 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
   dim3 grid((unsigned)std::min<long long>(p.e.total_tiles, num_sms()));
   const int smem = Cfg::kSmemBytes + (NORM ? d.Cin * 8 : 0);   // NORM: the per-channel scale / shift table
   B200_REQUIRE(smem <= 227 * 1024, "conv3x3x3_tc: Cin %d is too wide for the operand normalisation table", d.Cin);
+  const ConvTcAffine aff{d.in_gamma, d.in_beta};
   if constexpr (ADD) {
     auto kern = conv3x3x3_tc_add_kernel<NT, BD>;
     B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, ConvTcAffine{c.in_gamma, c.in_beta}, c.add);
+    kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, aff, ConvTcAdd{(const __half*)d.add, d.add_ctot, d.add_coff});
     B200_LAUNCH_CHECK("conv3x3x3_tc_add_kernel");
   } else {
     auto kern = conv3x3x3_tc_kernel<NT, BD, NORM, RES>;
     // per-device attribute: set on every call (cheap), so a second GPU in the same process works
     B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, ConvTcAffine{c.in_gamma, c.in_beta});
+    kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, aff);
     B200_LAUNCH_CHECK("conv3x3x3_tc_kernel");
   }
   if (c.stats) {
@@ -597,9 +594,9 @@ constexpr int kAddCols = 192;
 template <int NT, int BD>
 static int launch_variant(const b200_conv_tc_desc& d, ConvTcCall& c) {
   if constexpr (BD * NT <= kAddCols) {
-    if (d.in_stats && c.has_add) return launch_conv_tc<NT, BD, true, false, true>(d, c);
+    if (d.add) return launch_conv_tc<NT, BD, true, false, true>(d, c);
   }
-  if (c.has_add) return set_err(B200_ERR_UNSUPPORTED, "conv3x3x3_tc_affine_add: no instantiation for NT %d, BD %d", NT, BD);
+  if (d.add) return set_err(B200_ERR_UNSUPPORTED, "conv3x3x3_tc: no epilogue-add instantiation for NT %d, BD %d", NT, BD);
   if (d.in_stats) return launch_conv_tc<NT, BD, true>(d, c);
   if constexpr (NT <= 128 && 2 * BD * NT <= 256) {
     if (d.res_w) return launch_conv_tc<NT, BD, false, true>(d, c);
@@ -612,7 +609,7 @@ static int dispatch_bd(const b200_conv_tc_desc& d, ConvTcCall& c) {
   // deeper CTA tiles amortise the halo and fuse more kd taps per MMA; the depth is bounded by the accumulators a consumer
   // thread can hold (BD * NT, twice that with the folded residual, <= 256 columns = 128 registers)
   const int res = d.res_w ? 2 : 1;
-  const int cols = c.has_add ? kAddCols : 256;
+  const int cols = d.add ? kAddCols : 256;
   if constexpr (NT * 4 <= 256) {
     if ((d.D % 4 == 0 || d.D >= 16) && 4 * NT * res <= cols) return launch_variant<NT, 4>(d, c);
   }
@@ -630,6 +627,13 @@ static int conv_tc_dispatch(const b200_conv_tc_desc& d, ConvTcCall& c) {
   B200_REQUIRE(d.out_ctot % 8 == 0 && d.out_coff % 8 == 0 && d.out_coff + d.Cout <= d.out_ctot, "conv3x3x3_tc: bad output channel slice");
   B200_REQUIRE(!d.in_stats || d.in_act == 0 || d.in_act == 1 || d.in_act == 3, "conv3x3x3_tc: in_act must be none, leaky-relu or relu");
   B200_REQUIRE(!d.in_stats || d.in_act != 1 || (d.in_slope >= 0.f && d.in_slope <= 1.f), "conv3x3x3_tc: in_slope must lie in [0, 1] (got %g)", (double)d.in_slope);
+  B200_REQUIRE(d.in_stats || !(d.in_gamma || d.in_beta), "conv3x3x3_tc: affine parameters of the operand normalisation without in_stats");
+  if (d.add) {
+    B200_REQUIRE(d.in_stats && !d.res_w, "conv3x3x3_tc: the epilogue add needs in_stats (the operand normalisation) and no folded residual");
+    B200_REQUIRE(d.add_ctot % 8 == 0 && d.add_coff % 8 == 0 && d.add_coff >= 0 && d.add_coff + d.Cout <= d.add_ctot,
+                 "conv3x3x3_tc: bad channel slice of the added tensor");
+    B200_REQUIRE((reinterpret_cast<uintptr_t>(d.add) & 15) == 0, "conv3x3x3_tc: the added tensor must be 16-byte aligned");
+  }
   if (d.res_w) {
     B200_REQUIRE(!d.in_stats, "conv3x3x3_tc: the folded residual convolution and the operand normalisation are exclusive");
     B200_REQUIRE(d.res_y && d.Cout <= 128, "conv3x3x3_tc: the folded residual convolution needs res_y and Cout <= 128 (got %d)", d.Cout);
@@ -651,74 +655,27 @@ static int conv_tc_dispatch(const b200_conv_tc_desc& d, ConvTcCall& c) {
 
 extern "C" long long b200_conv3x3x3_tc_workspace_bytes(const b200_conv_tc_desc* desc) {
   if (!desc) return -1;
-  ConvTcCall c{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1, nullptr, nullptr, ConvTcAdd{nullptr, 0, 0}, false};
+  ConvTcCall c{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1};
   if (conv_tc_dispatch(*desc, c)) return -1;
   return c.ws_bytes;
-}
-
-// the epilogue add may run shallower tiles than the plain kernel (BD * NT <= kAddCols), so its statistics scratch can be larger
-extern "C" long long b200_conv3x3x3_tc_affine_add_workspace_bytes(const b200_conv_tc_desc* desc) {
-  if (!desc) return -1;
-  ConvTcCall c{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1, nullptr, nullptr, ConvTcAdd{nullptr, 0, 0}, true};
-  if (conv_tc_dispatch(*desc, c)) return -1;
-  return c.ws_bytes;
-}
-
-static int conv3x3x3_tc_run(const b200_conv_tc_desc* desc, const float* in_gamma, const float* in_beta, const void* x, const void* packed_w,
-                            const float* bias, void* y, float* stats, void* workspace, void* stream,
-                            ConvTcAdd add = ConvTcAdd{nullptr, 0, 0}) {
-  B200_REQUIRE(desc && x && packed_w && y, "conv3x3x3_tc: null pointer");
-  B200_REQUIRE(!(stats || (desc && desc->res_stats)) || workspace, "conv3x3x3_tc: statistics need the workspace of b200_conv3x3x3_tc_workspace_bytes()");
-  B200_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
-               (reinterpret_cast<uintptr_t>(packed_w) & 15) == 0, "conv3x3x3_tc: pointers must be 16-byte aligned");
-  B200_REQUIRE(desc->in_stats || !(in_gamma || in_beta), "conv3x3x3_tc: affine parameters of the operand normalisation without in_stats");
-  ConvTcCall c{x, packed_w, bias, y, stats, workspace, (cudaStream_t)stream, 0, 0, in_gamma, in_beta, add, add.x != nullptr};
-  return conv_tc_dispatch(*desc, c);
 }
 
 extern "C" int b200_conv3x3x3_tc(const b200_conv_tc_desc* desc, const void* x, const void* packed_w, const float* bias,
                                  void* y, float* stats, void* workspace, void* stream) {
-  return conv3x3x3_tc_run(desc, nullptr, nullptr, x, packed_w, bias, y, stats, workspace, stream);
+  B200_REQUIRE(desc && x && packed_w && y, "conv3x3x3_tc: null pointer");
+  B200_REQUIRE(!(stats || desc->res_stats) || workspace, "conv3x3x3_tc: statistics need the workspace of b200_conv3x3x3_tc_workspace_bytes()");
+  B200_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
+               (reinterpret_cast<uintptr_t>(packed_w) & 15) == 0, "conv3x3x3_tc: pointers must be 16-byte aligned");
+  ConvTcCall c{x, packed_w, bias, y, stats, workspace, (cudaStream_t)stream, 0, 0};
+  return conv_tc_dispatch(*desc, c);
 }
 
-extern "C" int b200_conv3x3x3_tc_affine(const b200_conv_tc_desc* desc, const float* in_gamma, const float* in_beta, const void* x,
-                                        const void* packed_w, const float* bias, void* y, float* stats, void* workspace, void* stream) {
-  return conv3x3x3_tc_run(desc, in_gamma, in_beta, x, packed_w, bias, y, stats, workspace, stream);
-}
-
-extern "C" int b200_conv3x3x3_tc_affine_add(const b200_conv_tc_desc* desc, const float* in_gamma, const float* in_beta, const void* x,
-                                            const void* packed_w, const float* bias, const void* add, int add_ctot, int add_coff, void* y,
-                                            float* stats, void* workspace, void* stream) {
-  B200_REQUIRE(desc && add, "conv3x3x3_tc_affine_add: null pointer");
-  B200_REQUIRE(desc->in_stats && !desc->res_w, "conv3x3x3_tc_affine_add: needs in_stats (the operand normalisation) and no folded residual");
-  B200_REQUIRE(add_ctot % 8 == 0 && add_coff % 8 == 0 && add_coff >= 0 && add_coff + desc->Cout <= add_ctot,
-               "conv3x3x3_tc_affine_add: bad channel slice of the added tensor");
-  B200_REQUIRE((reinterpret_cast<uintptr_t>(add) & 15) == 0, "conv3x3x3_tc_affine_add: pointers must be 16-byte aligned");
-  return conv3x3x3_tc_run(desc, in_gamma, in_beta, x, packed_w, bias, y, stats, workspace, stream,
-                          ConvTcAdd{(const __half*)add, add_ctot, add_coff});
-}
-
-// y = act(instnorm(x) [+ instnorm?(res)]) with optional affine parameters per norm: the body of b200_norm_act_nc8 and
-// b200_norm_act_affine_nc8
-static int norm_act_nc8_launch(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats, float eps,
-                               const void* res, int res_ctot, int res_coff, const float* res_stats, int act, float slope, void* y,
-                               int y_ctot, int y_coff, const float* gamma, const float* beta, const float* res_gamma,
-                               const float* res_beta, void* stream) {
-  B200_REQUIRE(x && y, "norm_act_nc8: null pointer");
-  B200_REQUIRE(C % 8 == 0 && x_ctot % 8 == 0 && x_coff % 8 == 0 && y_ctot % 8 == 0 && y_coff % 8 == 0, "norm_act_nc8: channels must be multiples of 8");
-  B200_REQUIRE(act == 0 || act == 1 || act == 3, "norm_act_nc8: activation must be none, leaky-relu or relu");
-  B200_REQUIRE(stats || !(gamma || beta), "norm_act_nc8: affine parameters without statistics");
-  B200_REQUIRE(res_stats || !(res_gamma || res_beta), "norm_act_nc8: residual affine parameters without residual statistics");
-  if ((long long)N * C * S == 0) return B200_OK;
-  NormActNc8P p;
-  p.x = (const __half*)x; p.y = (__half*)y; p.res = (const __half*)res; p.C = C;
-  p.x_ctot = x_ctot; p.x_coff = x_coff; p.y_ctot = y_ctot; p.y_coff = y_coff; p.r_ctot = res_ctot; p.r_coff = res_coff;
-  p.S = S; p.stats = stats; p.res_stats = res_stats; p.eps = eps; p.act = act; p.slope = slope;
-  p.raw = nullptr; p.raw_stats = nullptr; p.raw_w = nullptr;
-  long long want = (long long)num_sms() * 16 / ((long long)N * (C / 8)) + 1;
-  dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(want, (S + 255) / 256)), C / 8, N);
-  const NormAffineP a{gamma, beta, res_gamma, res_beta};
-  if (gamma || beta || res_gamma || res_beta) norm_act_nc8_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
+// sizes the grid and launches norm_act_nc8_kernel: the body of b200_norm_act_nc8 and b200_norm_act_cin1res_nc8
+static int norm_act_nc8_launch(const NormActNc8P& p, int N, const NormAffineP& a, void* stream) {
+  if ((long long)N * p.C * p.S == 0) return B200_OK;
+  long long want = (long long)num_sms() * 16 / ((long long)N * (p.C / 8)) + 1;
+  dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(want, (p.S + 255) / 256)), p.C / 8, N);
+  if (a.gamma || a.beta || a.res_gamma || a.res_beta) norm_act_nc8_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
   else norm_act_nc8_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
   B200_LAUNCH_CHECK("norm_act_nc8_kernel");
   return B200_OK;
@@ -726,17 +683,16 @@ static int norm_act_nc8_launch(const void* x, int x_ctot, int x_coff, int N, int
 
 extern "C" int b200_norm_act_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats,
                                  float eps, const void* res, int res_ctot, int res_coff, const float* res_stats, int act,
-                                 float slope, void* y, int y_ctot, int y_coff, void* stream) {
-  return norm_act_nc8_launch(x, x_ctot, x_coff, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, act, slope, y, y_ctot, y_coff,
-                             nullptr, nullptr, nullptr, nullptr, stream);
-}
-
-extern "C" int b200_norm_act_affine_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats,
-                                        float eps, const void* res, int res_ctot, int res_coff, const float* res_stats, int act,
-                                        float slope, void* y, int y_ctot, int y_coff, const float* gamma, const float* beta,
-                                        const float* res_gamma, const float* res_beta, void* stream) {
-  return norm_act_nc8_launch(x, x_ctot, x_coff, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, act, slope, y, y_ctot, y_coff,
-                             gamma, beta, res_gamma, res_beta, stream);
+                                 float slope, void* y, int y_ctot, int y_coff, const float* gamma, const float* beta,
+                                 const float* res_gamma, const float* res_beta, void* stream) {
+  B200_REQUIRE(x && y, "norm_act_nc8: null pointer");
+  B200_REQUIRE(C % 8 == 0 && x_ctot % 8 == 0 && x_coff % 8 == 0 && y_ctot % 8 == 0 && y_coff % 8 == 0, "norm_act_nc8: channels must be multiples of 8");
+  B200_REQUIRE(act == 0 || act == 1 || act == 3, "norm_act_nc8: activation must be none, leaky-relu or relu");
+  B200_REQUIRE(stats || !(gamma || beta), "norm_act_nc8: affine parameters without statistics");
+  B200_REQUIRE(res_stats || !(res_gamma || res_beta), "norm_act_nc8: residual affine parameters without residual statistics");
+  const NormActNc8P p{(const __half*)x, (__half*)y, (const __half*)res, C, x_ctot, x_coff, y_ctot, y_coff, res_ctot, res_coff, S,
+                      stats, res_stats, eps, act, slope, nullptr, nullptr, nullptr};
+  return norm_act_nc8_launch(p, N, NormAffineP{gamma, beta, res_gamma, res_beta}, stream);
 }
 
 extern "C" int b200_norm_act_cin1res_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats,
@@ -745,15 +701,7 @@ extern "C" int b200_norm_act_cin1res_nc8(const void* x, int x_ctot, int x_coff, 
   B200_REQUIRE(x && y && stats && raw && raw_stats && raw_weight, "norm_act_cin1res_nc8: null pointer");
   B200_REQUIRE(C % 8 == 0 && x_ctot % 8 == 0 && x_coff % 8 == 0 && y_ctot % 8 == 0 && y_coff % 8 == 0, "norm_act_cin1res_nc8: channels must be multiples of 8");
   B200_REQUIRE(act == 0 || act == 1 || act == 3, "norm_act_cin1res_nc8: activation must be none, leaky-relu or relu");
-  if ((long long)N * C * S == 0) return B200_OK;
-  NormActNc8P p;
-  p.x = (const __half*)x; p.y = (__half*)y; p.res = nullptr; p.C = C;
-  p.x_ctot = x_ctot; p.x_coff = x_coff; p.y_ctot = y_ctot; p.y_coff = y_coff; p.r_ctot = 0; p.r_coff = 0;
-  p.S = S; p.stats = stats; p.res_stats = nullptr; p.eps = eps; p.act = act; p.slope = slope;
-  p.raw = (const __half*)raw; p.raw_stats = raw_stats; p.raw_w = raw_weight;
-  long long want = (long long)num_sms() * 16 / ((long long)N * (C / 8)) + 1;
-  dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(want, (S + 255) / 256)), C / 8, N);
-  norm_act_nc8_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(p, NormAffineP{nullptr, nullptr, nullptr, nullptr});
-  B200_LAUNCH_CHECK("norm_act_nc8_kernel");
-  return B200_OK;
+  const NormActNc8P p{(const __half*)x, (__half*)y, nullptr, C, x_ctot, x_coff, y_ctot, y_coff, 0, 0, S,
+                      stats, nullptr, eps, act, slope, (const __half*)raw, raw_stats, raw_weight};
+  return norm_act_nc8_launch(p, N, NormAffineP{nullptr, nullptr, nullptr, nullptr}, stream);
 }

@@ -643,11 +643,10 @@ __global__ void __launch_bounds__(256) head_conv_norm_nc8_kernel(HeadNormP p) {
 
 using namespace b200;
 
-// the body of b200_head_conv_norm_nc8 and b200_head_conv_norm_affine_nc8
-static int head_conv_norm_nc8_launch(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
-                                     int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
-                                     const float* bias, int Cout, void* y, int out_dtype, const float* gamma, const float* beta,
-                                     void* stream) {
+extern "C" int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
+                                       int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
+                                       const float* bias, int Cout, void* y, int out_dtype, const float* gamma, const float* beta,
+                                       void* stream) {
   B200_REQUIRE(x && y && weight && stats, "head_conv_norm_nc8: null pointer");
   B200_REQUIRE(C % 8 == 0 && Cout >= 1 && Cout <= 16, "head_conv_norm_nc8: C must be a multiple of 8 and Cout <= 16 (got %d, %d)", C, Cout);
   B200_REQUIRE(!res || (res_ctot % 8 == 0 && res_coff % 8 == 0 && res_coff + C <= res_ctot), "head_conv_norm_nc8: bad residual channel slice");
@@ -667,21 +666,6 @@ static int head_conv_norm_nc8_launch(const void* x, int N, int C, long long S, c
 #undef LHN
   B200_LAUNCH_CHECK("head_conv_norm_nc8_kernel");
   return B200_OK;
-}
-
-extern "C" int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
-                                       int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
-                                       const float* bias, int Cout, void* y, int out_dtype, void* stream) {
-  return head_conv_norm_nc8_launch(x, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, slope, weight, bias, Cout, y, out_dtype,
-                                   nullptr, nullptr, stream);
-}
-
-extern "C" int b200_head_conv_norm_affine_nc8(const void* x, int N, int C, long long S, const float* stats, float eps, const void* res,
-                                              int res_ctot, int res_coff, const float* res_stats, float slope, const float* weight,
-                                              const float* bias, int Cout, void* y, int out_dtype, const float* gamma,
-                                              const float* beta, void* stream) {
-  return head_conv_norm_nc8_launch(x, N, C, S, stats, eps, res, res_ctot, res_coff, res_stats, slope, weight, bias, Cout, y, out_dtype,
-                                   gamma, beta, stream);
 }
 
 extern "C" int b200_layernorm_nc8(const void* x, int N, int C, long long S_in, const int32_t* src, long long S_out,

@@ -10,9 +10,9 @@ It owns what those networks share:
   * the packed-weight cache, the channel-padded input stem, and the residual / basic blocks, transposed convolutions and output
     head of the CNN parts.  The block helpers accept any module with the `conv1.conv` / `conv2.conv` / optional `conv3.conv`,
     `norm1/2/3` and `lrelu` structure of UnetResBlock / UnetBasicBlock (dynunet_block.py:25-177; kernel 3, stride 1 or 2,
-    InstanceNorm with or without affine parameters, LeakyReLU).  eps, gamma / beta and the slope are read from the block, so the
-    non-affine blocks of the transformer segmenters (eps 1e-5, slope 0.01) call exactly the entry points and arguments they
-    did before the affine variants existed.
+    InstanceNorm with or without affine parameters, LeakyReLU).  eps, gamma / beta and the slope are read from the block; the
+    non-affine blocks of the transformer segmenters (eps 1e-5, slope 0.01) pass no gamma / beta, so their kernels run the
+    non-affine instantiations.
 
 A network calls `self._tc_setup()` in its constructor and supplies `_forward_tc` and `_forward_generic`."""
 from __future__ import annotations

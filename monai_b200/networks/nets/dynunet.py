@@ -14,7 +14,7 @@ Two forwards, chosen from the input and the configuration (DESIGN.md §8.4):
     slope in [0, 1], out_channels <= 16; dropout inactive at call time): `_forward_tc`, the whole network on fp16 channel-blocked
     (NC8) buffers and Hopper tensor cores -- `b200_conv3x3x3_tc` for the stride-1 3x3x3 convolutions (the previous norm +
     LeakyReLU applied on the operand load), `b200_conv_gather_tc` for the stride-2 ones, `b200_gemm_tc` for the transposed
-    convolutions, the affine output head `b200_head_conv_norm_affine_nc8` -- replayed from a CUDA graph per input shape;
+    convolutions, the output head `b200_head_conv_norm_nc8` with the affine norm -- replayed from a CUDA graph per input shape;
   * everything else (fp32 input, anisotropic plans, other norms): `_forward_generic`, the fp32-faithful generic kernels.
 """
 from __future__ import annotations

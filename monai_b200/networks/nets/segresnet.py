@@ -11,7 +11,7 @@ Two forwards, chosen from the input and the configuration (DESIGN.md §8.4):
     dropout inactive at call time): `_forward_tc`, the whole network on fp16 channel-blocked (NC8) buffers and Hopper tensor
     cores -- every 3x3x3 convolution on `b200_conv3x3x3_tc` with the previous GroupNorm + activation applied on its operand load
     (`b200_group_stats` folds the per-channel sums of the conv epilogues into group sums), the residual add in conv2's epilogue
-    (`b200_conv3x3x3_tc_affine_add`), the stride-2 convolutions on `b200_conv_gather_tc`, the 1x1x1 / transposed convolutions on
+    (the `add` of `b200_conv3x3x3_tc`), the stride-2 convolutions on `b200_conv_gather_tc`, the 1x1x1 / transposed convolutions on
     `b200_gemm_tc`, upsample + skip add in one pass (`b200_upsample_add_nc8`) -- replayed from a CUDA graph per input shape;
   * everything else (fp32 input, 2-D, init_filters % 16 != 0, BatchNorm, other activations): `_forward_generic`, the
     fp32-faithful generic kernels.

@@ -1,6 +1,6 @@
-"""The fp16 tensor-core forward of DynUNet and the affine InstanceNorm of the NC8 kernels (b200_norm_act_affine_nc8,
-b200_conv3x3x3_tc_affine, b200_head_conv_norm_affine_nc8), against torch and against fixtures of the real reference
-(tests/golden/dynunet_tc.npz, configurations in tc_cases.py)."""
+"""The fp16 tensor-core forward of DynUNet and the affine InstanceNorm of the NC8 kernels (b200_norm_act_nc8 with gamma / beta,
+b200_conv3x3x3_tc with in_gamma / in_beta, b200_head_conv_norm_nc8 with gamma / beta), against torch and against fixtures of the
+real reference (tests/golden/dynunet_tc.npz, configurations in tc_cases.py)."""
 import os
 
 import numpy as np
@@ -81,16 +81,18 @@ def test_norm_act_affine_nc8_vs_torch(act, slope, with_res):
     assert err <= 2.0**-10 * float(ref.abs().max()) + 1e-3, err   # fp16 storage of the result
 
 
-def test_norm_act_affine_symbol_with_null_params_matches_old_symbol():
+def test_norm_act_unit_affine_params_match_no_params():
+    """gamma = 1, beta = 0 (and the same for the residual) runs the affine instantiation, which gives the bits of the non-affine one,
+    for x alone and for x + residual."""
     N, C, sp = 2, 24, (5, 6, 7)
     x = K.pack_nc8(torch.randn(N, C, *sp, generator=_gen(11)).half().to(DEV))
     r = K.pack_nc8(torch.randn(N, C, *sp, generator=_gen(12)).half().to(DEV))
     st, rst = _stats(K.unpack_nc8(x, dtype=torch.float32)), _stats(K.unpack_nc8(r, dtype=torch.float32))
-    old = K.norm_act_nc8(x, C, st, res=r, res_stats=rst, act=L.ACT_LEAKY, slope=0.01)
-    new = K.NC8(N, C, sp, DEV)
-    K._call("norm_act_affine_nc8", L.ptr(x.buf), x.C, 0, N, C, x.S, L.ptr(st), 1e-5, L.ptr(r.buf), r.C, 0, L.ptr(rst), L.ACT_LEAKY, 0.01,
-            L.ptr(new.buf), new.C, 0, None, None, None, None, L.stream_ptr(torch.device(DEV)))
-    assert torch.equal(old.buf, new.buf)
+    one, zero = torch.ones(C, device=DEV), torch.zeros(C, device=DEV)
+    for res_kw, res_affine in (({}, {}), (dict(res=r, res_stats=rst), dict(res_gamma=one, res_beta=zero))):
+        plain = K.norm_act_nc8(x, C, st, act=L.ACT_LEAKY, slope=0.01, **res_kw)
+        unit = K.norm_act_nc8(x, C, st, act=L.ACT_LEAKY, slope=0.01, gamma=one, beta=zero, **res_kw, **res_affine)
+        assert torch.equal(plain.buf, unit.buf), sorted(res_kw)
 
 
 @pytest.mark.parametrize("Cin,Cout,N,D", [(32, 32, 1, 16), (32, 64, 1, 6), (64, 128, 1, 3), (64, 320, 1, 2), (48, 32, 1, 1), (32, 64, 3, 24)])

@@ -1,5 +1,6 @@
-"""The fp16 tensor-core forward of SegResNet and its kernels (b200_group_stats, b200_conv3x3x3_tc_affine_add, b200_upsample_add_nc8),
-against torch and against fixtures of the real reference (tests/golden/segresnet_tc.npz, configurations in tc_cases.py)."""
+"""The fp16 tensor-core forward of SegResNet and its kernels (b200_group_stats, the epilogue add of b200_conv3x3x3_tc,
+b200_upsample_add_nc8), against torch and against fixtures of the real reference (tests/golden/segresnet_tc.npz, configurations in
+tc_cases.py)."""
 import ctypes as C
 import os
 
@@ -107,13 +108,18 @@ def test_conv_tc_affine_add_vs_torch(Cout, N, D):
     assert torch.equal(y2.buf, y.buf) and torch.equal(yst2, yst)
 
 
-def test_conv_tc_affine_add_sizes_its_own_workspace():
+def test_conv_tc_workspace_query_sizes_the_epilogue_add():
     """At 128 channels the add runs BD = 1 tiles where the plain kernel runs BD = 2: on a small volume (fewer tiles than SMs) its
-    statistics need more partial rows, which its own workspace query accounts for."""
-    d = L.ConvTcDesc(1, 32, 128, 5, 20, 24, 32, 0, 128, 0, 1, 1e-5, 3, 0.0, None, None, 0, 0, None)   # in_stats: any non-NULL value
+    statistics need more partial rows, which the workspace query sizes from the descriptor's add."""
+    d = L.ConvTcDesc(N=1, Cin=32, Cout=128, D=5, H=20, W=24, in_ctot=32, out_ctot=128, in_stats=16, in_eps=1e-5, in_act=L.ACT_RELU,
+                     add_ctot=128)   # in_stats, add: any non-NULL 16-byte-aligned value
     lib = L.load()
-    plain, add = lib.b200_conv3x3x3_tc_workspace_bytes(C.byref(d)), lib.b200_conv3x3x3_tc_affine_add_workspace_bytes(C.byref(d))
-    assert plain > 0 and add > plain, (plain, add)
+    plain = lib.b200_conv3x3x3_tc_workspace_bytes(C.byref(d))
+    d.add = 16
+    with_add = lib.b200_conv3x3x3_tc_workspace_bytes(C.byref(d))
+    assert with_add > plain > 0, (plain, with_add)
+    d.in_stats = None
+    assert lib.b200_conv3x3x3_tc_workspace_bytes(C.byref(d)) == -1   # the add needs the operand normalisation
 
 
 def test_conv_tc_affine_add_channel_slice():

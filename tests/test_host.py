@@ -63,11 +63,14 @@ def test_abi_exports_every_declared_symbol():
     assert _lib.load().b200_abi_version() == _lib.ABI_VERSION
 
 
-def test_struct_layouts_match_header_sizes():
+def test_struct_layouts_match_abi3_header():
     # sanity: ctypes mirrors must be at least as large as the packed field sum and 8-byte aligned
     assert ctypes.sizeof(_lib.BlendDesc) % 8 == 0
     assert ctypes.sizeof(_lib.ConvDesc) == 21 * 4 + 4 + 16
-    assert ctypes.sizeof(_lib.ConvTcDesc) == 96   # 10 ints, in_stats (offset 40), eps, act, slope, pad; res_w, res_y, res_ctot, res_coff, res_stats
+    # 10 ints, in_stats (offset 40), eps, act, slope, pad; res_w, res_y, res_ctot, res_coff, res_stats; in_gamma, in_beta, add, add_ctot, add_coff
+    assert ctypes.sizeof(_lib.ConvTcDesc) == 128
+    assert (_lib.ConvTcDesc.in_stats.offset, _lib.ConvTcDesc.res_w.offset, _lib.ConvTcDesc.in_gamma.offset, _lib.ConvTcDesc.add.offset,
+            _lib.ConvTcDesc.add_coff.offset) == (40, 64, 96, 112, 124)
 
 
 def test_argument_validation_matches_reference():
