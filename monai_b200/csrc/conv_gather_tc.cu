@@ -230,6 +230,12 @@ __global__ void __launch_bounds__(384, 1) conv_gather_tc_kernel(CgParams p) {
         if (wid == 0 && lane == 0) tc::mbar_arrive(&empty[s]);
         if (++s == kCgStages) { s = 0; ph ^= 1; }
       }
+      // a parity class without live taps (a transposed conv with k < stride, e.g. the odd outputs of k1 s2) runs no MMA,
+      // and only its first MMA would have cleared the accumulators: its outputs are the bias alone, as in torch
+      if (units == 0) {
+#pragma unroll
+        for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+      }
       const long long cv = (long long)rt * 128 + q * 32 + lane;
       bool ok = cv < coarse;
       long long orow = 0;
