@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 3
+#define B200_ABI_VERSION 4
 
 /* ---- library ---------------------------------------------------------------------------------------- */
 int b200_abi_version(void);
@@ -229,10 +229,23 @@ long long b200_conv3x3x3_tc_workspace_bytes(const b200_conv_tc_desc* desc);
 int b200_conv3x3x3_tc(const b200_conv_tc_desc* desc, const void* x, const void* packed_w, const float* bias,
                       void* y, float* stats, void* workspace, void* stream);
 
+/* Stride-1 convolution with a 3x3 kernel in one plane and 1 along the third axis (ABI 4): `axis` = 0, 1 or 2 names the axis of
+ * size 1 -- kernels [1,3,3], [3,1,3] and [3,3,1], zero padding (k - 1) / 2 per axis -- the high-resolution convolutions of
+ * anisotropic nnU-Net / DynUNet plans.  The same kernel as b200_conv3x3x3_tc without the dead taps; its result equals
+ * b200_conv3x3x3_tc with the weight zero-padded to 3x3x3, bit for bit.  Takes the b200_conv_tc_desc of b200_conv3x3x3_tc with the
+ * plain and the operand-normalising forms (in_stats, optionally in_gamma / in_beta); res_w and add return B200_ERR_UNSUPPORTED and
+ * the workspace query returns -1 for them.  The weight is the Conv3d weight [Cout,Cin,kd,kh,kw] float32 (device) with the axis of
+ * size 1 (9 * Cin * Cout values). */
+long long b200_conv3x3_tc_weight_bytes(int Cin, int Cout);
+int b200_conv3x3_tc_pack_weight(const float* w, int Cin, int Cout, int axis, void* packed, void* stream);
+long long b200_conv3x3_tc_workspace_bytes(const b200_conv_tc_desc* desc, int axis);
+int b200_conv3x3_tc(const b200_conv_tc_desc* desc, int axis, const void* x, const void* packed_w, const float* bias,
+                    void* y, float* stats, void* workspace, void* stream);
+
 typedef struct b200_conv_gather_desc {
   int N, Cin, Cout;         /* Cin % 16 == 0; Cout arbitrary for NCDHW output, % 8 == 0 for NC8 output */
   int Di, Hi, Wi, Do, Ho, Wo;
-  int k, stride, pad;       /* cubic kernel k <= 3, stride 1 or 2, zero padding */
+  int k[3], stride[3], pad[3];   /* per axis (d, h, w; ABI 4): kernel <= 3, stride 1 or 2, zero padding < 3 */
   int transposed;           /* 0: Conv3d weight [Cout,Cin,k,k,k]; 1: ConvTranspose3d weight [Cin,Cout,k,k,k] */
   int in_ctot, in_coff;     /* x = channels [in_coff, in_coff+Cin) of an NC8 buffer */
   int out_ctot, out_coff;   /* NC8 destination slice (out_layout 0) */
@@ -240,9 +253,11 @@ typedef struct b200_conv_gather_desc {
   int out_dtype;
 } b200_conv_gather_desc;
 
-/* General Conv3d / ConvTranspose3d (k <= 3, stride <= 2) as an implicit GEMM on wgmma with a cp.async im2col
- * producer -- the stride-2 and transposed 3x3x3 layers of UNet (monai/networks/nets/unet.py:150-182).  Weights are
- * packed per (N tile, parity class, live tap, 16-channel slice); stats as in b200_conv3x3x3_tc. */
+/* General Conv3d / ConvTranspose3d (kernel <= 3, stride <= 2, per axis) as an implicit GEMM on wgmma with a cp.async im2col
+ * producer -- the stride-2 and transposed 3x3x3 layers of UNet (monai/networks/nets/unet.py:150-182), and the anisotropic
+ * strided convolutions ([1,3,3] stride [1,2,2], ...) and transposed convolutions (kernel = stride = [1,2,2], ...) of DynUNet.  A
+ * transposed convolution runs sd*sh*sw parity classes.  Weights (Conv3d [Cout,Cin,kd,kh,kw] / ConvTranspose3d [Cin,Cout,kd,kh,kw])
+ * are packed per (N tile, parity class, live tap, 16-channel slice); stats as in b200_conv3x3x3_tc. */
 long long b200_conv_gather_tc_weight_bytes(const b200_conv_gather_desc* desc);
 int b200_conv_gather_tc_pack_weight(const b200_conv_gather_desc* desc, const float* w, void* packed, void* stream);
 long long b200_conv_gather_tc_workspace_bytes(const b200_conv_gather_desc* desc);   /* statistics scratch, as for b200_conv3x3x3_tc */

@@ -6,6 +6,7 @@ sm_90a kernel reached through ctypes.  All functions require CUDA tensors.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import weakref
 from typing import Sequence
 
@@ -601,6 +602,53 @@ def conv3x3x3_tc(
     return out, stats
 
 
+def conv3x3_tc_pack_weight(weight: torch.Tensor, axis: int) -> torch.Tensor:
+    """Pack a Conv3d weight [Cout, Cin, kd, kh, kw] whose kernel is 1 along `axis` and 3 along the other two for conv3x3_tc."""
+    L.require_cuda(weight)
+    Cout, Cin = weight.shape[:2]
+    want = tuple(1 if a == axis else 3 for a in range(3))
+    if tuple(weight.shape[2:]) != want:
+        raise ValueError(f"conv3x3_tc: a weight of kernel {want} for axis {axis}, got {tuple(weight.shape[2:])}")
+    nbytes = L.load().b200_conv3x3_tc_weight_bytes(Cin, Cout)
+    if nbytes < 0:
+        raise ValueError(f"conv3x3_tc needs Cin, Cout multiples of 16, got {Cin}, {Cout}")
+    w32 = weight.detach().float().contiguous()
+    packed = torch.empty(nbytes // 2, device=weight.device, dtype=torch.float16)
+    _call("conv3x3_tc_pack_weight", L.ptr(w32), Cin, Cout, int(axis), L.ptr(packed), L.stream_ptr(weight.device))
+    return packed
+
+
+def conv3x3_tc(
+    x: NC8, packed_w: torch.Tensor, Cin: int, Cout: int, axis: int, in_coff: int = 0, bias: torch.Tensor | None = None,
+    out: NC8 | None = None, out_coff: int = 0, want_stats: bool = False,
+    in_norm: tuple[torch.Tensor, float, int, float] | None = None,
+    in_affine: tuple[torch.Tensor | None, torch.Tensor | None] | None = None,
+):
+    """Stride-1 convolution whose kernel is 1 along `axis` and 3 along the other two (padding 0 / 1 / 1 accordingly), e.g. the
+    [1, 3, 3] convolutions of anisotropic DynUNet plans.  `in_norm` / `in_affine` as in conv3x3x3_tc.  Returns (out, stats)."""
+    if out is None:
+        out = NC8(x.N, Cout, x.sp, x.buf.device)
+    dev = x.buf.device
+    stats = torch.empty((x.N * Cout, 2), device=dev, dtype=torch.float32) if want_stats else None
+    b32 = _f32c(bias)
+    d = L.ConvTcDesc(N=x.N, Cin=Cin, Cout=Cout, D=x.sp[0], H=x.sp[1], W=x.sp[2], in_ctot=x.C, in_coff=in_coff, out_ctot=out.C,
+                     out_coff=out_coff)
+    if in_norm is not None:
+        st, eps, act, slope = in_norm
+        if st.dtype != torch.float32 or st.numel() != x.N * Cin * 2 or not st.is_contiguous() or st.device != dev:
+            raise ValueError("conv3x3_tc: in_norm statistics must be a contiguous float32 [N*Cin, 2] tensor on the input's device")
+        d.in_stats, d.in_eps, d.in_act, d.in_slope = L.ptr(st), float(eps), int(act), float(slope)
+    g32, be32 = (_f32c(t) for t in (in_affine or (None, None)))
+    if (g32 is not None or be32 is not None) and in_norm is None:
+        raise ValueError("conv3x3_tc: in_affine needs in_norm")
+    d.in_gamma, d.in_beta = L.ptr(g32), L.ptr(be32)
+    ws = _ws(L.load().b200_conv3x3_tc_workspace_bytes(C.byref(d), int(axis)), dev) if want_stats else None
+    _call("conv3x3_tc", C.byref(d), int(axis), L.ptr(x.buf), L.ptr(packed_w), L.ptr(b32), L.ptr(out.buf), L.ptr(stats), L.ptr(ws),
+          L.stream_ptr(dev), flops=2.0 * x.N * x.S * Cin * Cout * 9, nbytes=float(x.N * x.S * (Cin + Cout) * 2) + _nb(packed_w),
+          label="conv3x3_tc_affine" if g32 is not None or be32 is not None else "conv3x3_tc")
+    return out, stats
+
+
 def norm_act_cin1res_nc8(x: NC8, C_: int, stats: torch.Tensor, raw: torch.Tensor, raw_stats: torch.Tensor, raw_weight: torch.Tensor,
                          act: int = L.ACT_NONE, slope: float = 0.0, out: NC8 | None = None, out_coff: int = 0, eps: float = 1e-5) -> NC8:
     """act(instnorm(x) + instnorm(conv1x1x1(raw))) for a ONE-channel `raw` [N,1,*sp] fp16: the residual branch is an affine
@@ -891,17 +939,23 @@ def head_conv_norm_nc8(x: NC8, stats: torch.Tensor, res: NC8 | None, res_coff: i
     return y
 
 
+_I3 = C.c_int * 3   # the per-axis (d, h, w) fields of b200_conv_gather_desc
+
+
 def _cg_desc(x_sp, N, Cin, Cout, k, stride, pad, transposed, output_padding, in_ctot, in_coff, out_ctot, out_coff, out_layout, out_dtype):
-    sp_out = conv_out_shape(x_sp, (k,) * 3, (stride,) * 3, (pad,) * 3, transposed, (output_padding,) * 3)
-    return L.ConvGatherDesc(N, Cin, Cout, x_sp[0], x_sp[1], x_sp[2], sp_out[0], sp_out[1], sp_out[2], k, stride, pad, int(transposed),
-                            in_ctot, in_coff, out_ctot, out_coff, out_layout, out_dtype), sp_out
+    k, stride, pad, output_padding = _t3(k), _t3(stride), _t3(pad), _t3(output_padding)
+    sp_out = conv_out_shape(x_sp, k, stride, pad, transposed, output_padding)
+    return L.ConvGatherDesc(N, Cin, Cout, x_sp[0], x_sp[1], x_sp[2], sp_out[0], sp_out[1], sp_out[2], _I3(*k), _I3(*stride), _I3(*pad),
+                            int(transposed), in_ctot, in_coff, out_ctot, out_coff, out_layout, out_dtype), sp_out
 
 
-def conv_gather_tc_pack_weight(weight: torch.Tensor, k: int, stride: int, pad: int, transposed: bool) -> torch.Tensor:
-    """Pack a Conv3d [Cout,Cin,k,k,k] / ConvTranspose3d [Cin,Cout,k,k,k] weight for conv_gather_tc."""
+def conv_gather_tc_pack_weight(weight: torch.Tensor, k, stride, pad, transposed: bool) -> torch.Tensor:
+    """Pack a Conv3d [Cout,Cin,kd,kh,kw] / ConvTranspose3d [Cin,Cout,kd,kh,kw] weight for conv_gather_tc; `k`, `stride` and `pad`
+    are ints or (d, h, w) triples."""
     L.require_cuda(weight)
     Cin, Cout = (weight.shape[0], weight.shape[1]) if transposed else (weight.shape[1], weight.shape[0])
-    d, _ = _cg_desc((8, 8, 8), 1, Cin, Cout, k, stride, pad, transposed, stride - 1 if transposed else 0, Cin, 0, (Cout + 7) // 8 * 8, 0, 1, L.DT_F16)
+    op = tuple(s - 1 for s in _t3(stride)) if transposed else 0
+    d, _ = _cg_desc((8, 8, 8), 1, Cin, Cout, k, stride, pad, transposed, op, Cin, 0, (Cout + 7) // 8 * 8, 0, 1, L.DT_F16)
     nbytes = L.load().b200_conv_gather_tc_weight_bytes(C.byref(d))
     if nbytes < 0:
         raise ValueError(f"conv_gather_tc needs Cin % 16 == 0, kernel <= 3, stride <= 2 (got Cin={Cin}, k={k}, stride={stride})")
@@ -912,11 +966,12 @@ def conv_gather_tc_pack_weight(weight: torch.Tensor, k: int, stride: int, pad: i
 
 
 def conv_gather_tc(
-    x: NC8, packed_w: torch.Tensor, Cin: int, Cout: int, k: int, stride: int, pad: int, transposed: bool = False, output_padding: int = 0,
+    x: NC8, packed_w: torch.Tensor, Cin: int, Cout: int, k, stride, pad, transposed: bool = False, output_padding=0,
     in_coff: int = 0, bias: torch.Tensor | None = None, out: "NC8 | torch.Tensor | None" = None, out_coff: int = 0,
     ncdhw_dtype: torch.dtype | None = None, want_stats: bool = False,
 ):
-    """Conv3d / ConvTranspose3d on tensor cores.  Returns (NC8 | NCDHW tensor, stats)."""
+    """Conv3d / ConvTranspose3d on tensor cores; `k`, `stride`, `pad` and `output_padding` are ints or (d, h, w) triples.  Returns
+    (NC8 | NCDHW tensor, stats)."""
     layout = 0 if ncdhw_dtype is None else 1
     d, sp_out = _cg_desc(x.sp, x.N, Cin, Cout, k, stride, pad, transposed, output_padding, x.C, in_coff,
                          (out.C if isinstance(out, NC8) else (Cout + 7) // 8 * 8), out_coff, layout, L.dt(ncdhw_dtype) if layout else L.DT_F16)
@@ -925,7 +980,7 @@ def conv_gather_tc(
         d.out_ctot = out.C if layout == 0 else d.out_ctot
     stats = torch.empty((x.N * Cout, 2), device=x.buf.device, dtype=torch.float32) if want_stats else None
     b32 = _f32c(bias)
-    taps = k**3 if not transposed else (k**3) / (stride**3)
+    taps = math.prod(d.k) / (math.prod(d.stride) if transposed else 1)
     ws = _ws(L.load().b200_conv_gather_tc_workspace_bytes(C.byref(d)), x.buf.device) if want_stats else None
     _call("conv_gather_tc", C.byref(d), L.ptr(x.buf), L.ptr(packed_w), L.ptr(b32), L.ptr(out.buf if layout == 0 else out), L.ptr(stats), L.ptr(ws),
           L.stream_ptr(x.buf.device), flops=2.0 * x.N * sp_out[0] * sp_out[1] * sp_out[2] * Cin * Cout * taps,

@@ -14,7 +14,7 @@ import torch
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = _HERE / "lib" / "libmonai_b200.so"
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 DT_F32, DT_F16 = 0, 1
 _DT = {torch.float32: DT_F32, torch.float16: DT_F16}
 
@@ -57,9 +57,8 @@ class ConvTcDesc(C.Structure):
 
 
 class ConvGatherDesc(C.Structure):
-    _fields_ = [(n, i32) for n in (
-        "N", "Cin", "Cout", "Di", "Hi", "Wi", "Do", "Ho", "Wo", "k", "stride", "pad", "transposed", "in_ctot", "in_coff",
-        "out_ctot", "out_coff", "out_layout", "out_dtype")]
+    _fields_ = ([(n, i32) for n in ("N", "Cin", "Cout", "Di", "Hi", "Wi", "Do", "Ho", "Wo")] + [(n, i32 * 3) for n in ("k", "stride", "pad")]
+                + [(n, i32) for n in ("transposed", "in_ctot", "in_coff", "out_ctot", "out_coff", "out_layout", "out_dtype")])
 
 
 class GemmTcDesc(C.Structure):
@@ -97,6 +96,10 @@ SIGNATURES = {
     "b200_conv3x3x3_tc_pack_weight": (i32, [vp, i32, i32, vp, vp]),
     "b200_conv3x3x3_tc_workspace_bytes": (i64, [C.POINTER(ConvTcDesc)]),
     "b200_conv3x3x3_tc": (i32, [C.POINTER(ConvTcDesc), vp, vp, vp, vp, vp, vp, vp]),
+    "b200_conv3x3_tc_weight_bytes": (i64, [i32, i32]),
+    "b200_conv3x3_tc_pack_weight": (i32, [vp, i32, i32, i32, vp, vp]),
+    "b200_conv3x3_tc_workspace_bytes": (i64, [C.POINTER(ConvTcDesc), i32]),
+    "b200_conv3x3_tc": (i32, [C.POINTER(ConvTcDesc), i32, vp, vp, vp, vp, vp, vp, vp]),
     "b200_conv_gather_tc_weight_bytes": (i64, [C.POINTER(ConvGatherDesc)]),
     "b200_conv_gather_tc_pack_weight": (i32, [C.POINTER(ConvGatherDesc), vp, vp, vp]),
     "b200_conv_gather_tc_workspace_bytes": (i64, [C.POINTER(ConvGatherDesc)]),

@@ -1,9 +1,10 @@
-// General 3-D convolution / transposed convolution (kernel <= 3, any stride) as an implicit GEMM on Hopper wgmma tensor
-// cores with a software im2col producer (SURVEY.md §8 row a8: the stride-2 Conv3d and ConvTranspose3d(k3, s2) layers
-// of UNet, monai/networks/nets/unet.py:150-182 via monai/networks/blocks/convolutions.py:131-152).
+// General 3-D convolution / transposed convolution (kernel <= 3, stride <= 2, per axis) as an implicit GEMM on Hopper wgmma
+// tensor cores with a software im2col producer (SURVEY.md §8 row a8: the stride-2 Conv3d and ConvTranspose3d(k3, s2) layers
+// of UNet, monai/networks/nets/unet.py:150-182 via monai/networks/blocks/convolutions.py:131-152; the anisotropic strided and
+// transposed convolutions of DynUNet).
 //
 // GEMM view: rows = 128 output voxels of ONE parity class (forward conv: a single class; transposed conv with
-// stride s: s^3 classes, so that every row of a tile uses the same set of live taps -- no work is spent on taps that
+// stride (sd, sh, sw): sd*sh*sw classes, so that every row of a tile uses the same set of live taps -- no work is spent on taps that
 // cannot reach an output voxel), columns = NT output channels, K = (live taps) x Cin walked in units of 16 channels.
 // Producer warps (128 threads, one GEMM row each) gather the 16-channel vectors of the tap's input voxel with
 // cp.async (16-byte pieces of the NC8 layout, zero-filled outside the volume = zero padding) straight into the wgmma
@@ -29,7 +30,7 @@ struct CgParams {
   const __half* x; const __half* w; const float* bias; void* y;
   StatsPartials sp;           // deterministic InstanceNorm partial sums (stats.cuh)
   int NT, cout_pad;
-  int ncls, mul;              // classes; input coordinate = coarse * mul + tap offset
+  int ncls, mul[3];           // classes; input coordinate = coarse * mul + tap offset (d, h, w)
   int Dc, Hc, Wc;             // coarse extent of one class
   int cls_ntaps[8], cls_unit_off[8];
   CgTap taps[8][27];
@@ -38,26 +39,26 @@ struct CgParams {
 
 // enumerate the live taps of every parity class (shared by the pack kernel and the conv kernel)
 static void cg_build_taps(const b200_conv_gather_desc& d, CgParams& p) {
-  const int k = d.k, s = d.stride, pad = d.pad;
-  p.ncls = d.transposed ? s * s * s : 1;
-  p.mul = d.transposed ? 1 : s;
+  const int* k = d.k; const int* s = d.stride; const int* pad = d.pad;
+  p.ncls = d.transposed ? s[0] * s[1] * s[2] : 1;
+  for (int a = 0; a < 3; ++a) p.mul[a] = d.transposed ? 1 : s[a];
+  auto md = [](int v, int m) { return ((v % m) + m) % m; };
+  auto fdiv = [md](int v, int m) { return (v - md(v, m)) / m; };
   int off = 0;
   for (int c = 0; c < p.ncls; ++c) {
-    const int px = c % s, py = (c / s) % s, pz = c / (s * s);
+    const int px = c % s[2], py = (c / s[2]) % s[1], pz = c / (s[2] * s[1]);
     int nt = 0;
-    for (int kz = 0; kz < k; ++kz)
-      for (int ky = 0; ky < k; ++ky)
-        for (int kx = 0; kx < k; ++kx) {
+    for (int kz = 0; kz < k[0]; ++kz)
+      for (int ky = 0; ky < k[1]; ++ky)
+        for (int kx = 0; kx < k[2]; ++kx) {
           CgTap t;
-          t.id = (unsigned char)((kz * k + ky) * k + kx);
+          t.id = (unsigned char)((kz * k[1] + ky) * k[2] + kx);
           if (d.transposed) {
-            const int tz = pz + pad - kz, ty = py + pad - ky, tx = px + pad - kx;
-            auto divisible = [s](int v) { return ((v % s) + s) % s == 0; };
-            if (!divisible(tz) || !divisible(ty) || !divisible(tx)) continue;
-            auto fdiv = [s](int v) { return (v - (((v % s) + s) % s)) / s; };
-            t.dz = (signed char)fdiv(tz); t.dy = (signed char)fdiv(ty); t.dx = (signed char)fdiv(tx);
+            const int tz = pz + pad[0] - kz, ty = py + pad[1] - ky, tx = px + pad[2] - kx;
+            if (md(tz, s[0]) || md(ty, s[1]) || md(tx, s[2])) continue;
+            t.dz = (signed char)fdiv(tz, s[0]); t.dy = (signed char)fdiv(ty, s[1]); t.dx = (signed char)fdiv(tx, s[2]);
           } else {
-            t.dz = (signed char)(kz - pad); t.dy = (signed char)(ky - pad); t.dx = (signed char)(kx - pad);
+            t.dz = (signed char)(kz - pad[0]); t.dy = (signed char)(ky - pad[1]); t.dx = (signed char)(kx - pad[2]);
           }
           p.taps[c][nt++] = t;
         }
@@ -71,7 +72,7 @@ static void cg_build_taps(const b200_conv_gather_desc& d, CgParams& p) {
 // packed layout: [nt][unit][khalf][NT/8][8][8], unit = cls_unit_off[cls] + tap_index_in_class * (Cin/16) + kc
 __global__ void cg_pack_weight_kernel(const float* __restrict__ w, __half* __restrict__ out, CgParams p) {
   const b200_conv_gather_desc& d = p.d;
-  const int NT = p.NT, kcs = d.Cin / 16, ktaps = d.k * d.k * d.k;
+  const int NT = p.NT, kcs = d.Cin / 16, ktaps = d.k[0] * d.k[1] * d.k[2];
   const long long total = (long long)(p.cout_pad / NT) * p.units_total * NT * 16;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     long long r = i;
@@ -146,7 +147,7 @@ __global__ void __launch_bounds__(384, 1) conv_gather_tc_kernel(CgParams p) {
       const long long cv = (long long)rt * 128 + r;
       const bool row_ok = cv < coarse;
       const int cx = row_ok ? (int)(cv % p.Wc) : 0, cy = row_ok ? (int)((cv / p.Wc) % p.Hc) : 0, cz = row_ok ? (int)(cv / ((long long)p.Wc * p.Hc)) : 0;
-      const int bz = cz * p.mul, by = cy * p.mul, bx = cx * p.mul;
+      const int bz = cz * p.mul[0], by = cy * p.mul[1], bx = cx * p.mul[2];
       const int units = p.cls_ntaps[cls] * kcs;
       const __half* xn = p.x + ((long long)n * (d.in_ctot / 8) + d.in_coff / 8) * Si * 8;
       const __half* wbase = p.w + ((long long)nt * p.units_total + p.cls_unit_off[cls]) * (NT * 16);
@@ -242,8 +243,8 @@ __global__ void __launch_bounds__(384, 1) conv_gather_tc_kernel(CgParams p) {
       if (ok) {
         int ox = (int)(cv % p.Wc), oy = (int)((cv / p.Wc) % p.Hc), oz = (int)(cv / ((long long)p.Wc * p.Hc));
         if (d.transposed) {
-          const int s_ = d.stride;
-          ox = ox * s_ + cls % s_; oy = oy * s_ + (cls / s_) % s_; oz = oz * s_ + cls / (s_ * s_);
+          const int sd = d.stride[0], sh = d.stride[1], sw = d.stride[2];
+          ox = ox * sw + cls % sw; oy = oy * sh + (cls / sw) % sh; oz = oz * sd + cls / (sw * sh);
         }
         ok = oz < d.Do && oy < d.Ho && ox < d.Wo;
         orow = ((long long)oz * d.Ho + oy) * d.Wo + ox;
@@ -321,7 +322,9 @@ static int cg_launch(const CgParams& p, long long total_tiles, cudaStream_t st) 
 
 static int cg_setup(const b200_conv_gather_desc& d, CgParams& p) {
   B200_REQUIRE(d.N > 0 && d.Cin > 0 && d.Cin % 16 == 0 && d.Cout > 0, "conv_gather_tc: Cin must be a multiple of 16 (got %d)", d.Cin);
-  B200_REQUIRE(d.k >= 1 && d.k <= 3 && d.stride >= 1 && d.stride <= 2 && d.pad >= 0 && d.pad < 3, "conv_gather_tc: kernel <= 3, stride <= 2");
+  for (int a = 0; a < 3; ++a)
+    B200_REQUIRE(d.k[a] >= 1 && d.k[a] <= 3 && d.stride[a] >= 1 && d.stride[a] <= 2 && d.pad[a] >= 0 && d.pad[a] < 3,
+                 "conv_gather_tc: kernel <= 3, stride <= 2, pad < 3 on every axis");
   B200_REQUIRE(d.in_ctot % 8 == 0 && d.in_coff % 8 == 0 && d.in_coff + d.Cin <= d.in_ctot, "conv_gather_tc: bad input channel slice");
   B200_REQUIRE(d.out_layout == 1 || (d.Cout % 8 == 0 && d.out_ctot % 8 == 0 && d.out_coff % 8 == 0 && d.out_coff + d.Cout <= d.out_ctot),
                "conv_gather_tc: NC8 output needs channel counts that are multiples of 8");
@@ -330,7 +333,7 @@ static int cg_setup(const b200_conv_gather_desc& d, CgParams& p) {
   p.NT = cg_nt(p.cout_pad);
   cg_build_taps(d, p);
   if (d.transposed) {
-    p.Dc = ceil_div(d.Do, d.stride); p.Hc = ceil_div(d.Ho, d.stride); p.Wc = ceil_div(d.Wo, d.stride);
+    p.Dc = ceil_div(d.Do, d.stride[0]); p.Hc = ceil_div(d.Ho, d.stride[1]); p.Wc = ceil_div(d.Wo, d.stride[2]);
   } else {
     p.Dc = d.Do; p.Hc = d.Ho; p.Wc = d.Wo;
   }
@@ -377,14 +380,15 @@ extern "C" int b200_conv_gather_tc(const b200_conv_gather_desc* desc, const void
   int rc = cg_setup(*desc, p);
   if (rc) return rc;
   const b200_conv_gather_desc& d = *desc;
-  // shape consistency with torch's conv arithmetic
-  if (!d.transposed) {
-    B200_REQUIRE(d.Do == (d.Di + 2 * d.pad - d.k) / d.stride + 1 && d.Ho == (d.Hi + 2 * d.pad - d.k) / d.stride + 1 &&
-                 d.Wo == (d.Wi + 2 * d.pad - d.k) / d.stride + 1, "conv_gather_tc: output shape does not match conv arithmetic");
-  } else {
-    const int lo_d = (d.Di - 1) * d.stride - 2 * d.pad + d.k, lo_h = (d.Hi - 1) * d.stride - 2 * d.pad + d.k, lo_w = (d.Wi - 1) * d.stride - 2 * d.pad + d.k;
-    B200_REQUIRE(d.Do >= lo_d && d.Do < lo_d + d.stride && d.Ho >= lo_h && d.Ho < lo_h + d.stride && d.Wo >= lo_w && d.Wo < lo_w + d.stride,
-                 "conv_gather_tc: output shape does not match transposed-conv arithmetic");
+  // shape consistency with torch's conv arithmetic, per axis
+  const int in_sp[3] = {d.Di, d.Hi, d.Wi}, out_sp[3] = {d.Do, d.Ho, d.Wo};
+  for (int a = 0; a < 3; ++a) {
+    if (!d.transposed) {
+      B200_REQUIRE(out_sp[a] == (in_sp[a] + 2 * d.pad[a] - d.k[a]) / d.stride[a] + 1, "conv_gather_tc: output shape does not match conv arithmetic");
+    } else {
+      const int lo = (in_sp[a] - 1) * d.stride[a] - 2 * d.pad[a] + d.k[a];
+      B200_REQUIRE(out_sp[a] >= lo && out_sp[a] < lo + d.stride[a], "conv_gather_tc: output shape does not match transposed-conv arithmetic");
+    }
   }
   p.x = (const __half*)x; p.w = (const __half*)packed_w; p.bias = bias; p.y = y;
   const long long coarse = (long long)p.Dc * p.Hc * p.Wc;

@@ -78,7 +78,9 @@ __global__ void __launch_bounds__(256) unpack_nc8_kernel(const __half* __restric
 
 // ----------------------------------------------------------------------------------------------------------
 // weight packing: Conv3d weight [Cout][Cin][27] fp32 -> [nt][kc][kh][kw][khalf][kd = 2,1,0][NT/8][8 cout][8 k] fp16
-// (one K-major B image of 3*NT rows per (kh, kw): rows of kd = 2 first, so a kd range is a contiguous row range)
+// (one K-major B image of 3*NT rows per (kh, kw): rows of kd = 2 first, so a kd range is a contiguous row range).
+// The one-plane 3x3 kernels of b200_conv3x3_tc (axis = the kernel axis of size 1) pack the same image without the dead taps:
+// axis 0 keeps NT rows (kd = 1) per (kh, kw), axes 1 and 2 keep the 3 live (kh, kw) of the 9.  axis -1 = 3x3x3.
 // ----------------------------------------------------------------------------------------------------------
 __host__ __device__ inline int conv_tc_nt(int Cout) {
   if (Cout <= 128) return Cout;
@@ -90,22 +92,28 @@ __host__ __device__ inline int conv_tc_nt(int Cout) {
   return 16;
 }
 
-__global__ void conv_tc_pack_weight_kernel(const float* __restrict__ w, __half* __restrict__ out, int Cin, int Cout, int NT) {
-  const long long total = (long long)Cout * Cin * 27;
+__host__ __device__ inline int conv_tc_kd_rows(int axis) { return axis == 0 ? 1 : 3; }   // kd taps per (kh, kw) image
+__host__ __device__ inline int conv_tc_taps(int axis) { return axis > 0 ? 3 : 9; }       // (kh, kw) images per K slice
+
+__global__ void conv_tc_pack_weight_kernel(const float* __restrict__ w, __half* __restrict__ out, int Cin, int Cout, int NT, int axis) {
+  const int nkd = conv_tc_kd_rows(axis), ntap = conv_tc_taps(axis);
+  const int KD = axis == 0 ? 1 : 3, KH = axis == 1 ? 1 : 3, KW = axis == 2 ? 1 : 3;   // extents of the source weight
+  const long long total = (long long)Cout * Cin * nkd * ntap;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     long long r = i;
     const int kk = (int)(r % 8); r /= 8;
     const int row = (int)(r % 8); r /= 8;
     const int g = (int)(r % (NT / 8)); r /= (NT / 8);
-    const int kd = 2 - (int)(r % 3); r /= 3;
+    const int kd = KD - 1 - (int)(r % nkd); r /= nkd;
     const int khalf = (int)(r % 2); r /= 2;
-    const int t9 = (int)(r % 9); r /= 9;    // kh*3 + kw
+    const int ti = (int)(r % ntap); r /= ntap;    // kh*3 + kw (3x3x3, axis 0), kw (axis 1), kh (axis 2)
     const int kc = (int)(r % (Cin / 16)); r /= (Cin / 16);
     const int nt = (int)r;
+    const int kh = axis == 1 ? 0 : (axis == 2 ? ti : ti / 3), kw = axis == 1 ? ti : (axis == 2 ? 0 : ti % 3);
     const int cout = nt * NT + g * 8 + row;
     const int cin = kc * 16 + khalf * 8 + kk;
-    const int tap = kd * 9 + t9;
-    out[i] = __float2half_rn(w[((long long)cout * Cin + cin) * 27 + tap]);
+    const int tap = (kd * KH + kh) * KW + kw;
+    out[i] = __float2half_rn(w[((long long)cout * Cin + cin) * (KD * KH * KW) + tap]);
   }
 }
 
@@ -114,12 +122,19 @@ __global__ void conv_tc_pack_weight_kernel(const float* __restrict__ w, __half* 
 // ----------------------------------------------------------------------------------------------------------
 constexpr int kHH = kTH + 2, kHW = kTW + 2;      // halo patch (kTH x kTW output patch: conv_epi.cuh)
 
-template <int NT, int BD, bool RES = false>
+// kernel forms of the body: the 3x3x3 convolution, and the one-plane 3x3 convolutions of b200_conv3x3_tc -- kernel 1 along D
+// (no depth halo, one kd tap per (kh, kw)), or kernel 1 along H or W (3 of the 9 (kh, kw) taps; which axis is a kernel argument)
+constexpr int kForm333 = 0, kFormD1 = 1, kFormHW1 = 2;
+
+template <int NT, int BD, bool RES = false, int KF = kForm333>
 struct ConvTcCfg {
-  static constexpr int kPlanes = BD + 2;
+  static constexpr int kPlanes = KF == kFormD1 ? BD : BD + 2;
+  static constexpr int kDHalo = KF == kFormD1 ? 0 : 1;          // input planes staged in front of the first output plane
+  static constexpr int kKd = KF == kFormD1 ? 1 : 3;             // kd taps per (kh, kw) image
+  static constexpr int kTaps = KF == kFormHW1 ? 3 : 9;          // (kh, kw) images per K slice
   static constexpr int kChunkBytes = kPlanes * kHH * kHW * 16;   // one 8-channel chunk of the halo tile
   static constexpr int kABytes = 2 * kChunkBytes;                // 16 input channels
-  static constexpr int kBTapBytes = 3 * NT * 32;                 // one (kh, kw): the three kd taps stacked along N, 3*NT x 16 fp16
+  static constexpr int kBTapBytes = kKd * NT * 32;               // one (kh, kw): the kd taps stacked along N, kKd*NT x 16 fp16
   // weight ring: one (kh, kw) tap image per stage, ~44 KB in flight so a bulk copy has > 1 us to land before its
   // MMAs are due
   static constexpr int kSB = (45056 / kBTapBytes) > 9 ? 9 : ((45056 / kBTapBytes) < 3 ? 3 : (45056 / kBTapBytes));
@@ -172,12 +187,17 @@ struct ConvTcAdd { const __half* x; int ctot, coff; };
 // are those of the sum -- conv2 plus the identity of a pre-activation residual block (SegResNet's ResBlock,
 // monai/networks/blocks/segresnet_block.py:83-94).  The body is shared by conv3x3x3_tc_kernel (ADD = false: the code it always
 // had) and conv3x3x3_tc_add_kernel.
-template <int NT, int BD, bool NORM, bool RES, bool ADD>
+//
+// KF (kernel form): kForm333, or a one-plane 3x3 kernel of b200_conv3x3_tc (see kFormD1 / kFormHW1; `axis` = 1 or 2 names the
+// axis of size 1 of kFormHW1).  The live MMAs of each accumulator run in the order of the 3x3x3 form, so a one-plane kernel gives the
+// bits of the 3x3x3 form with zero-padded weights.
+template <int NT, int BD, bool NORM, bool RES, bool ADD, int KF = kForm333>
 __device__ __forceinline__ void conv3x3x3_tc_body(const CUtensorMap& tmap, const ConvTcParams& p, const ConvTcAffine& aff,
-                                                  const ConvTcAdd& add) {
-  using Cfg = ConvTcCfg<NT, BD, RES>;
+                                                  const ConvTcAdd& add, int axis = 0) {
+  using Cfg = ConvTcCfg<NT, BD, RES, KF>;
   static_assert(!(NORM && RES), "the residual fold is used by conv1, the operand normalisation by conv2");
   static_assert(!ADD || (NORM && !RES), "the epilogue add is a variant of the operand-normalising instantiations");
+  static_assert(KF == kForm333 || !(RES || ADD), "the one-plane kernels have the plain and the operand-normalising forms only");
   constexpr int kSA = Cfg::kSA, kSB = Cfg::kSB;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = tc::align_smem128(smem_raw);   // keeps the shared address space (LDS/STS, not generic LD/ST)
@@ -217,11 +237,11 @@ __device__ __forceinline__ void conv3x3x3_tc_body(const CUtensorMap& tmap, const
       int sa = 0, sb = 0, sr = 0; uint32_t pa = 0, pb = 0, pr = 0;
       for (long long t = blockIdx.x; t < p.e.total_tiles; t += gridDim.x) {
         const ConvTile c = conv_tile<BD>(p.e, t);
-        const __half* wbase = p.w + (long long)c.nt * num_kc * 9 * (Cfg::kBTapBytes / 2);
+        const __half* wbase = p.w + (long long)c.nt * num_kc * Cfg::kTaps * (Cfg::kBTapBytes / 2);
         for (int kc = 0; kc < num_kc; ++kc) {
           tc::mbar_wait(&empty_a[sa], pa ^ 1);
           tc::mbar_arrive_expect_tx(&full_a[sa], Cfg::kABytes);
-          tc::tma_load_5d(smem_a + sa * Cfg::kABytes, &tmap, &full_a[sa], (c.w0 - 1) * 8, c.h0 - 1, c.d0 - 1,
+          tc::tma_load_5d(smem_a + sa * Cfg::kABytes, &tmap, &full_a[sa], (c.w0 - 1) * 8, c.h0 - 1, c.d0 - Cfg::kDHalo,
                           (d.in_coff + kc * 16) / 8, c.n);
           if (++sa == kSA) { sa = 0; pa ^= 1; }
           if constexpr (RES) {
@@ -230,10 +250,10 @@ __device__ __forceinline__ void conv3x3x3_tc_body(const CUtensorMap& tmap, const
             tc::bulk_load(smem_r + sr * Cfg::kRBytes, p.res_w + ((long long)c.nt * num_kc + kc) * (Cfg::kRBytes / 2), Cfg::kRBytes, &full_r[sr]);
             if (++sr == Cfg::kSR) { sr = 0; pr ^= 1; }
           }
-          for (int t9 = 0; t9 < 9; ++t9) {
+          for (int t9 = 0; t9 < Cfg::kTaps; ++t9) {
             tc::mbar_wait(&empty_b[sb], pb ^ 1);
             tc::mbar_arrive_expect_tx(&full_b[sb], Cfg::kBTapBytes);
-            tc::bulk_load(smem_b + sb * Cfg::kBTapBytes, wbase + ((long long)kc * 9 + t9) * (Cfg::kBTapBytes / 2), Cfg::kBTapBytes,
+            tc::bulk_load(smem_b + sb * Cfg::kBTapBytes, wbase + ((long long)kc * Cfg::kTaps + t9) * (Cfg::kBTapBytes / 2), Cfg::kBTapBytes,
                           &full_b[sb]);
             if (++sb == kSB) { sb = 0; pb ^= 1; }
           }
@@ -266,19 +286,29 @@ __device__ __forceinline__ void conv3x3x3_tc_body(const CUtensorMap& tmap, const
         tc::mbar_wait(&full_b[sb], pb);
         const uint32_t b_tap = tc::smem_u32(smem_b + sb * Cfg::kBTapBytes);
         tc::wg_fence();
-        tc::static_for<0, BD + 2>([&](auto ipc) {
-          constexpr int ip = decltype(ipc)::value;
-          constexpr int kd_hi = ip < 2 ? ip : 2, kd_lo = ip - (BD - 1) > 0 ? ip - (BD - 1) : 0;
-          const uint32_t a_addr = a_base + ((ip * kHH + kh) * kHW + kw) * 16;
-          const uint64_t adesc = tc::make_desc_kmajor_noswz(a_addr, Cfg::kChunkBytes, kHW * 16);
-          tc::static_for<0, 3>([&](auto kdc) {
-            constexpr int kd = 2 - decltype(kdc)::value;
-            if constexpr (kd <= kd_hi && kd >= kd_lo) {
-              const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_tap + (2 - kd) * NT * 16, 3 * NT * 16, 128);
-              tc::wg_mma_ss<NT>(acc + (ip - kd) * NT / 2, adesc, bdesc, 1u, 128);
-            }
+        if constexpr (KF == kFormD1) {
+          // no depth halo: staged plane ip is output plane ip, and only the kd = 1 tap is live
+          const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_tap, NT * 16, 128);
+          tc::static_for<0, BD>([&](auto ipc) {
+            constexpr int ip = decltype(ipc)::value;
+            const uint64_t adesc = tc::make_desc_kmajor_noswz(a_base + ((ip * kHH + kh) * kHW + kw) * 16, Cfg::kChunkBytes, kHW * 16);
+            tc::wg_mma_ss<NT>(acc + ip * NT / 2, adesc, bdesc, 1u, 128);
           });
-        });
+        } else {
+          tc::static_for<0, BD + 2>([&](auto ipc) {
+            constexpr int ip = decltype(ipc)::value;
+            constexpr int kd_hi = ip < 2 ? ip : 2, kd_lo = ip - (BD - 1) > 0 ? ip - (BD - 1) : 0;
+            const uint32_t a_addr = a_base + ((ip * kHH + kh) * kHW + kw) * 16;
+            const uint64_t adesc = tc::make_desc_kmajor_noswz(a_addr, Cfg::kChunkBytes, kHW * 16);
+            tc::static_for<0, 3>([&](auto kdc) {
+              constexpr int kd = 2 - decltype(kdc)::value;
+              if constexpr (kd <= kd_hi && kd >= kd_lo) {
+                const uint64_t bdesc = tc::make_desc_kmajor_noswz(b_tap + (2 - kd) * NT * 16, 3 * NT * 16, 128);
+                tc::wg_mma_ss<NT>(acc + (ip - kd) * NT / 2, adesc, bdesc, 1u, 128);
+              }
+            });
+          });
+        }
         tc::wg_commit();
         tc::wg_wait<1>();
         if (prev_sb >= 0 && leader) tc::mbar_arrive(&empty_b[prev_sb]);
@@ -302,8 +332,13 @@ __device__ __forceinline__ void conv3x3x3_tc_body(const CUtensorMap& tmap, const
       for (int kc = 0; kc < num_kc; ++kc) {
         tc::mbar_wait(NORM ? &ready_a[sa] : &full_a[sa], pa);
         a_base = tc::smem_u32(smem_a + sa * Cfg::kABytes) + g * 8 * kHW * 16;   // rows 64.. = patch rows h0 + 8 ..
+        if constexpr (KF == kFormHW1) {
 #pragma unroll 1
-        for (int t9 = 0; t9 < 9; ++t9) tap(t9 / 3, t9 % 3);
+          for (int t = 0; t < 3; ++t) tap(axis == 1 ? 1 : t, axis == 1 ? t : 1);
+        } else {
+#pragma unroll 1
+          for (int t9 = 0; t9 < 9; ++t9) tap(t9 / 3, t9 % 3);
+        }
         if constexpr (RES) residual();
         tc::wg_wait<0>();
         tc::wg_fence_acc<Cfg::kAccSet / 2>(acc);
@@ -365,7 +400,7 @@ __device__ __forceinline__ void conv3x3x3_tc_body(const CUtensorMap& tmap, const
         if (col_in) {
 #pragma unroll 2
           for (int pz = 0; pz < Cfg::kPlanes; ++pz) {
-            if ((unsigned)(c.d0 - 1 + pz) >= (unsigned)d.D) continue;
+            if ((unsigned)(c.d0 - Cfg::kDHalo + pz) >= (unsigned)d.D) continue;
 #pragma unroll
             for (int i = 0; i < kHH / kRowT; ++i) {
               if ((unsigned)(c.h0 - 1 + py0 + kRowT * i) >= (unsigned)d.H) continue;
@@ -401,6 +436,13 @@ template <int NT, int BD, bool NORM, bool RES>
 __global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3_tc_kernel(const __grid_constant__ CUtensorMap tmap, ConvTcParams p,
                                                                                                   ConvTcAffine aff) {
   conv3x3x3_tc_body<NT, BD, NORM, RES, false>(tmap, p, aff, ConvTcAdd{nullptr, 0, 0});
+}
+
+// the one-plane 3x3 convolution (b200_conv3x3_tc): KF = kFormD1 or kFormHW1, plain or operand-normalising
+template <int NT, int BD, bool NORM, int KF>
+__global__ void __launch_bounds__(ConvTcCfg<NT, BD, false, KF>::kThreads, 1) conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmap, ConvTcParams p,
+                                                                                                   ConvTcAffine aff, int axis) {
+  conv3x3x3_tc_body<NT, BD, NORM, false, false, KF>(tmap, p, aff, ConvTcAdd{nullptr, 0, 0}, axis);
 }
 
 template <int NT, int BD>
@@ -513,7 +555,7 @@ extern "C" int b200_conv3x3x3_tc_pack_weight(const float* w, int Cin, int Cout, 
   B200_REQUIRE(Cin > 0 && Cout > 0 && Cin % 16 == 0 && Cout % 16 == 0, "conv3x3x3_tc: Cin and Cout must be multiples of 16 (got %d, %d)", Cin, Cout);
   const long long total = (long long)Cin * Cout * 27;
   const int blocks = (int)std::min<long long>((total + 255) / 256, 4096);
-  conv_tc_pack_weight_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, (__half*)packed, Cin, Cout, conv_tc_nt(Cout));
+  conv_tc_pack_weight_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, (__half*)packed, Cin, Cout, conv_tc_nt(Cout), -1);
   B200_LAUNCH_CHECK("conv_tc_pack_weight_kernel");
   return B200_OK;
 }
@@ -527,14 +569,16 @@ struct ConvTcGeom {
   }
 };
 
-// what a launch needs beyond the operands: mode 0 = run, mode 1 = only report the statistics workspace size
+// what a launch needs beyond the operands: mode 0 = run, mode 1 = only report the statistics workspace size.  axis: -1 for the
+// 3x3x3 convolution, else the kernel axis of size 1 of b200_conv3x3_tc.
 struct ConvTcCall {
   const void* x; const void* w; const float* bias; void* y; float* stats; void* ws; cudaStream_t st; long long ws_bytes; int query;
+  int axis;
 };
 
-template <int NT, int BD, bool NORM, bool RES = false, bool ADD = false>
+template <int NT, int BD, bool NORM, bool RES = false, bool ADD = false, int KF = kForm333>
 static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
-  using Cfg = ConvTcCfg<NT, BD, RES>;
+  using Cfg = ConvTcCfg<NT, BD, RES, KF>;
   ConvTcParams p;
   p.d = d; p.w = (const __half*)c.w; p.in_stats = (const float*)d.in_stats;
   ConvTcGeom<NT, BD>::fill(d, p.e);
@@ -550,7 +594,7 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
   const cuuint64_t S = (cuuint64_t)d.D * d.H * d.W;
   cuuint64_t gdim[5] = {(cuuint64_t)d.W * 8, (cuuint64_t)d.H, (cuuint64_t)d.D, (cuuint64_t)(d.in_ctot / 8), (cuuint64_t)d.N};
   cuuint64_t gstr[4] = {(cuuint64_t)d.W * 16, (cuuint64_t)d.H * d.W * 16, S * 16, S * 16 * (cuuint64_t)(d.in_ctot / 8)};
-  cuuint32_t box[5] = {(cuuint32_t)kHW * 8, (cuuint32_t)kHH, (cuuint32_t)(BD + 2), 2, 1};
+  cuuint32_t box[5] = {(cuuint32_t)kHW * 8, (cuuint32_t)kHH, (cuuint32_t)Cfg::kPlanes, 2, 1};
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   CUresult r = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(c.x), gdim, gstr, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -568,7 +612,12 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
   const int smem = Cfg::kSmemBytes + (NORM ? d.Cin * 8 : 0);   // NORM: the per-channel scale / shift table
   B200_REQUIRE(smem <= 227 * 1024, "conv3x3x3_tc: Cin %d is too wide for the operand normalisation table", d.Cin);
   const ConvTcAffine aff{d.in_gamma, d.in_beta};
-  if constexpr (ADD) {
+  if constexpr (KF != kForm333) {
+    auto kern = conv3x3_tc_kernel<NT, BD, NORM, KF>;
+    B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, aff, c.axis);
+    B200_LAUNCH_CHECK("conv3x3_tc_kernel");
+  } else if constexpr (ADD) {
     auto kern = conv3x3x3_tc_add_kernel<NT, BD>;
     B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, aff, ConvTcAdd{(const __half*)d.add, d.add_ctot, d.add_coff});
@@ -593,6 +642,10 @@ constexpr int kAddCols = 192;
 
 template <int NT, int BD>
 static int launch_variant(const b200_conv_tc_desc& d, ConvTcCall& c) {
+  if (c.axis >= 0) {   // b200_conv3x3_tc: plain or operand-normalising (its entry point rejects res_w and add)
+    if (c.axis == 0) return d.in_stats ? launch_conv_tc<NT, BD, true, false, false, kFormD1>(d, c) : launch_conv_tc<NT, BD, false, false, false, kFormD1>(d, c);
+    return d.in_stats ? launch_conv_tc<NT, BD, true, false, false, kFormHW1>(d, c) : launch_conv_tc<NT, BD, false, false, false, kFormHW1>(d, c);
+  }
   if constexpr (BD * NT <= kAddCols) {
     if (d.add) return launch_conv_tc<NT, BD, true, false, true>(d, c);
   }
@@ -655,7 +708,7 @@ static int conv_tc_dispatch(const b200_conv_tc_desc& d, ConvTcCall& c) {
 
 extern "C" long long b200_conv3x3x3_tc_workspace_bytes(const b200_conv_tc_desc* desc) {
   if (!desc) return -1;
-  ConvTcCall c{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1};
+  ConvTcCall c{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1, -1};
   if (conv_tc_dispatch(*desc, c)) return -1;
   return c.ws_bytes;
 }
@@ -666,8 +719,47 @@ extern "C" int b200_conv3x3x3_tc(const b200_conv_tc_desc* desc, const void* x, c
   B200_REQUIRE(!(stats || desc->res_stats) || workspace, "conv3x3x3_tc: statistics need the workspace of b200_conv3x3x3_tc_workspace_bytes()");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
                (reinterpret_cast<uintptr_t>(packed_w) & 15) == 0, "conv3x3x3_tc: pointers must be 16-byte aligned");
-  ConvTcCall c{x, packed_w, bias, y, stats, workspace, (cudaStream_t)stream, 0, 0};
+  ConvTcCall c{x, packed_w, bias, y, stats, workspace, (cudaStream_t)stream, 0, 0, -1};
   return conv_tc_dispatch(*desc, c);
+}
+
+extern "C" long long b200_conv3x3_tc_weight_bytes(int Cin, int Cout) {
+  if (Cin <= 0 || Cout <= 0 || Cin % 16 || Cout % 16) return -1;
+  return (long long)Cin * Cout * 9 * 2;
+}
+
+extern "C" int b200_conv3x3_tc_pack_weight(const float* w, int Cin, int Cout, int axis, void* packed, void* stream) {
+  B200_REQUIRE(w && packed, "conv3x3_tc_pack_weight: null pointer");
+  B200_REQUIRE(Cin > 0 && Cout > 0 && Cin % 16 == 0 && Cout % 16 == 0, "conv3x3_tc: Cin and Cout must be multiples of 16 (got %d, %d)", Cin, Cout);
+  B200_REQUIRE(axis >= 0 && axis <= 2, "conv3x3_tc: axis must be 0, 1 or 2 (got %d)", axis);
+  const long long total = (long long)Cin * Cout * 9;
+  const int blocks = (int)std::min<long long>((total + 255) / 256, 4096);
+  conv_tc_pack_weight_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, (__half*)packed, Cin, Cout, conv_tc_nt(Cout), axis);
+  B200_LAUNCH_CHECK("conv_tc_pack_weight_kernel");
+  return B200_OK;
+}
+
+static int conv3x3_tc_dispatch(const b200_conv_tc_desc& d, ConvTcCall& c) {
+  B200_REQUIRE(c.axis >= 0 && c.axis <= 2, "conv3x3_tc: axis must be 0, 1 or 2 (got %d)", c.axis);
+  if (d.res_w || d.add) return set_err(B200_ERR_UNSUPPORTED, "conv3x3_tc: the folded residual and the epilogue add are 3x3x3 forms only");
+  return conv_tc_dispatch(d, c);
+}
+
+extern "C" long long b200_conv3x3_tc_workspace_bytes(const b200_conv_tc_desc* desc, int axis) {
+  if (!desc) return -1;
+  ConvTcCall c{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1, axis};
+  if (conv3x3_tc_dispatch(*desc, c)) return -1;
+  return c.ws_bytes;
+}
+
+extern "C" int b200_conv3x3_tc(const b200_conv_tc_desc* desc, int axis, const void* x, const void* packed_w, const float* bias,
+                               void* y, float* stats, void* workspace, void* stream) {
+  B200_REQUIRE(desc && x && packed_w && y, "conv3x3_tc: null pointer");
+  B200_REQUIRE(!stats || workspace, "conv3x3_tc: statistics need the workspace of b200_conv3x3_tc_workspace_bytes()");
+  B200_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
+               (reinterpret_cast<uintptr_t>(packed_w) & 15) == 0, "conv3x3_tc: pointers must be 16-byte aligned");
+  ConvTcCall c{x, packed_w, bias, y, stats, workspace, (cudaStream_t)stream, 0, 0, axis};
+  return conv3x3_tc_dispatch(*desc, c);
 }
 
 // sizes the grid and launches norm_act_nc8_kernel: the body of b200_norm_act_nc8 and b200_norm_act_cin1res_nc8

@@ -9,8 +9,10 @@ It owns what those networks share:
     changes (`load_state_dict`, `.half()`).  MONAI_B200_GRAPH=0 disables the mechanism;
   * the packed-weight cache, the channel-padded input stem, and the residual / basic blocks, transposed convolutions and output
     head of the CNN parts.  The block helpers accept any module with the `conv1.conv` / `conv2.conv` / optional `conv3.conv`,
-    `norm1/2/3` and `lrelu` structure of UnetResBlock / UnetBasicBlock (dynunet_block.py:25-177; kernel 3, stride 1 or 2,
-    InstanceNorm with or without affine parameters, LeakyReLU).  eps, gamma / beta and the slope are read from the block; the
+    `norm1/2/3` and `lrelu` structure of UnetResBlock / UnetBasicBlock (dynunet_block.py:25-177; InstanceNorm with or without affine
+    parameters, LeakyReLU) and read kernel, stride and padding from the block's own convolutions: a stride-1 3x3x3 kernel runs on
+    conv3x3x3_tc, a stride-1 kernel of 3x3 in one plane and 1 along the third axis on conv3x3_tc, a kernel with stride 2 on any axis
+    on conv_gather_tc (per axis), and a stride-1 1x1x1 kernel on gemm_tc.  eps, gamma / beta and the slope are read from the block; the
     non-affine blocks of the transformer segmenters (eps 1e-5, slope 0.01) pass no gamma / beta, so their kernels run the
     non-affine instantiations.
 
@@ -149,9 +151,13 @@ class TcNet:
         params = [weight] + ([bias] if bias is not None else [])
         return self._cache.get(("qkvs", key, weight.device), params, build)
 
-    def _wg(self, conv: nn.Conv3d, key: str, k: int, stride: int, pad: int):
-        return self._cache.get(("wg", key, k, stride, pad, conv.weight.device), [conv.weight],
-                               lambda: K.conv_gather_tc_pack_weight(conv.weight, k, stride, pad, False))
+    def _w33(self, conv: nn.Conv3d, key: str, axis: int, cin_pad: int | None = None):
+        return self._cache.get(("w33", key, axis, cin_pad, conv.weight.device), [conv.weight],
+                               lambda: K.conv3x3_tc_pack_weight(self._pad_cin(conv.weight, cin_pad), axis))
+
+    def _wg(self, conv: nn.Module, key: str, k, stride, pad, transposed: bool = False):
+        return self._cache.get(("wg", key, k, stride, pad, transposed, conv.weight.device), [conv.weight],
+                               lambda: K.conv_gather_tc_pack_weight(conv.weight, k, stride, pad, transposed))
 
     # ------------------------------------------------------------------------------------------------- sub-graphs
     @staticmethod
@@ -174,22 +180,42 @@ class TcNet:
     def _slope(blk: nn.Module) -> float:
         return float(blk.lrelu.negative_slope)
 
-    def _conv1(self, x: K.NC8, cin: int, in_coff: int, blk: nn.Module, key: str, stride: int, cin_pad: int | None):
-        """conv1 of a block (raw output + statistics): 3x3x3 stride 1 on conv3x3x3_tc, stride 2 on conv_gather_tc."""
-        cout = blk.conv1.conv.out_channels
-        if stride == 2:
-            return K.conv_gather_tc(x, self._wg(blk.conv1.conv, key + ".c1", 3, 2, 1), cin, cout, 3, 2, 1, in_coff=in_coff, want_stats=True)
-        return K.conv3x3x3_tc(x, self._w3(blk.conv1.conv, key + ".c1", cin_pad), cin, cout, in_coff=in_coff, want_stats=True)
+    @staticmethod
+    def _strided(conv: nn.Module) -> bool:
+        return any(int(s) != 1 for s in conv.stride)
+
+    @staticmethod
+    def _one_plane_axis(conv: nn.Module) -> int:
+        """-1 for a 3x3x3 kernel, else the axis of size 1 of a 3x3 kernel in one plane (the kernels of conv3x3_tc)."""
+        k = tuple(int(i) for i in conv.kernel_size)
+        return -1 if k == (3, 3, 3) else k.index(1)
+
+    def _conv_s1(self, x: K.NC8, cin: int, conv: nn.Conv3d, key: str, cin_pad: int | None = None, **kw):
+        """A stride-1 convolution with a 3x3x3 kernel (conv3x3x3_tc) or a 3x3 kernel in one plane (conv3x3_tc)."""
+        axis = self._one_plane_axis(conv)
+        if axis < 0:
+            return K.conv3x3x3_tc(x, self._w3(conv, key, cin_pad), cin, conv.out_channels, **kw)
+        return K.conv3x3_tc(x, self._w33(conv, key, axis, cin_pad), cin, conv.out_channels, axis, **kw)
+
+    def _conv_strided(self, x: K.NC8, cin: int, in_coff: int, conv: nn.Conv3d, key: str):
+        """A convolution with stride 2 on some axis, on conv_gather_tc with the module's per-axis kernel, stride and padding."""
+        k, s, p = (tuple(int(i) for i in v) for v in (conv.kernel_size, conv.stride, conv.padding))
+        return K.conv_gather_tc(x, self._wg(conv, key, k, s, p), cin, conv.out_channels, k, s, p, in_coff=in_coff, want_stats=True)
+
+    def _conv1(self, x: K.NC8, cin: int, in_coff: int, blk: nn.Module, key: str, cin_pad: int | None):
+        """conv1 of a block (raw output + statistics)."""
+        if self._strided(blk.conv1.conv):
+            return self._conv_strided(x, cin, in_coff, blk.conv1.conv, key + ".c1")
+        return self._conv_s1(x, cin, blk.conv1.conv, key + ".c1", cin_pad, in_coff=in_coff, want_stats=True)
 
     def _conv2(self, y1: K.NC8, st1: torch.Tensor, blk: nn.Module, key: str):
         """conv2 with norm1 + lrelu of conv1's raw output applied on its operand load (no pass over the tensor in between)."""
-        cout = blk.conv2.conv.out_channels
         eps1, g1, b1 = self._norm(blk.norm1)
-        return K.conv3x3x3_tc(y1, self._w3(blk.conv2.conv, key + ".c2"), cout, cout, want_stats=True, in_norm=(st1, eps1, L.ACT_LEAKY, self._slope(blk)),
-                              in_affine=(g1, b1))
+        return self._conv_s1(y1, blk.conv2.conv.out_channels, blk.conv2.conv, key + ".c2", want_stats=True,
+                             in_norm=(st1, eps1, L.ACT_LEAKY, self._slope(blk)), in_affine=(g1, b1))
 
     def _basic_block(self, x: K.NC8, cin: int, in_coff: int, blk: nn.Module, key: str, out: K.NC8 | None = None, out_coff: int = 0,
-                     x_in_raw: torch.Tensor | None = None, defer_tail: bool = False, cin_pad: int | None = None, stride: int = 1):
+                     x_in_raw: torch.Tensor | None = None, defer_tail: bool = False, cin_pad: int | None = None):
         """UnetBasicBlock.forward (dynunet_block.py:165-177) on NC8 buffers: conv1, conv2 with norm1 + lrelu on its operand load,
         then norm2 + lrelu into `out` (may be a slice of a concat buffer).  With `defer_tail` the last step is NOT applied: the
         pieces are returned for `_tail_head` in the form `_res_block` returns them, without a residual."""
@@ -197,7 +223,7 @@ class TcNet:
         if x_in_raw is not None:  # single input channel: direct stem kernel on the raw NCDHW window
             y1, st1 = K.conv_cin1_nc8(x_in_raw, blk.conv1.conv.weight, None, 3, 1, 1, want_stats=True)
         else:
-            y1, st1 = self._conv1(x, cin, in_coff, blk, key, stride, cin_pad)
+            y1, st1 = self._conv1(x, cin, in_coff, blk, key, cin_pad)
         y2, st2 = self._conv2(y1, st1, blk, key)
         if defer_tail:
             return y2, st2, None, 0, None
@@ -208,10 +234,10 @@ class TcNet:
         return out
 
     def _res_block(self, x: K.NC8, cin: int, in_coff: int, blk: nn.Module, key: str, out: K.NC8 | None = None, out_coff: int = 0,
-                   x_in_raw: torch.Tensor | None = None, defer_tail: bool = False, cin_pad: int | None = None, stride: int = 1):
+                   x_in_raw: torch.Tensor | None = None, defer_tail: bool = False, cin_pad: int | None = None):
         """UnetResBlock.forward (dynunet_block.py:97-111) on NC8 buffers; `out` may be a slice of a concat buffer.  eps, the
-        (optional) affine parameters of norm1/2/3 and the LeakyReLU slope come from the block's modules.  stride 2: conv1 (k3 p1)
-        and conv3 (k1 p0) run on conv_gather_tc.
+        (optional) affine parameters of norm1/2/3 and the LeakyReLU slope come from the block's modules.  Strided: conv1 and conv3
+        (k1 p0) run on conv_gather_tc.
         With `defer_tail` the final norm2 + residual + lrelu is NOT applied: the pieces (y2, stats2, res, res_coff,
         res_stats) are returned so that the consumer (the output head) applies them on its operand load; that needs a
         non-affine norm3."""
@@ -223,13 +249,14 @@ class TcNet:
         folded = None
         if x_in_raw is not None:  # single input channel: direct stem kernels read the raw NCDHW window
             y1, st1 = K.conv_cin1_nc8(x_in_raw, blk.conv1.conv.weight, None, 3, 1, 1, want_stats=True)
-        elif stride == 1 and has3 and cout <= 128 and cin_pad is None and blk.conv3.conv.bias is None:
+        elif (has3 and not self._strided(blk.conv1.conv) and self._one_plane_axis(blk.conv1.conv) < 0 and cout <= 128 and cin_pad is None
+              and blk.conv3.conv.bias is None):
             # conv3 (1x1x1 residual branch) reads the same input as conv1: one launch produces both tensors and both statistics
             y1, st1, y3f, st3f = K.conv3x3x3_tc(x, self._w3(blk.conv1.conv, key + ".c1", cin_pad), cin, cout, in_coff=in_coff, want_stats=True,
                                                 res_w=self._wlin(blk.conv3.conv.weight, key + ".c3", cin_pad))
             folded = (y3f, st3f)
         else:
-            y1, st1 = self._conv1(x, cin, in_coff, blk, key, stride, cin_pad)
+            y1, st1 = self._conv1(x, cin, in_coff, blk, key, cin_pad)
         y2, st2 = self._conv2(y1, st1, blk, key)
         if has3:
             if (x_in_raw is not None and x_in_raw.dtype == torch.float16 and blk.conv3.conv.bias is None and not defer_tail
@@ -244,8 +271,8 @@ class TcNet:
                 y3, st3 = folded
             elif x_in_raw is not None:
                 y3, st3 = K.conv_cin1_nc8(x_in_raw, blk.conv3.conv.weight, None, 1, 1, 0, want_stats=True)
-            elif stride == 2:
-                y3, st3 = K.conv_gather_tc(x, self._wg(blk.conv3.conv, key + ".c3", 1, 2, 0), cin, cout, 1, 2, 0, in_coff=in_coff, want_stats=True)
+            elif self._strided(blk.conv3.conv):
+                y3, st3 = self._conv_strided(x, cin, in_coff, blk.conv3.conv, key + ".c3")
             else:
                 y3, st3 = K.gemm_tc(x, self._wlin(blk.conv3.conv.weight, key + ".c3", cin_pad), cin, cout, in_coff=in_coff, want_stats=True)
             if defer_tail:
@@ -263,7 +290,13 @@ class TcNet:
         return out
 
     def _up(self, x: K.NC8, cin: int, conv: nn.ConvTranspose3d, key: str, out: K.NC8 | None = None, out_coff: int = 0) -> K.NC8:
-        """ConvTranspose3d k2 s2 as a GEMM whose epilogue scatters to the 2x upsampled voxels (optionally a concat slice)."""
+        """ConvTranspose3d k2 s2 as a GEMM whose epilogue scatters to the 2x upsampled voxels (optionally a concat slice).  An
+        anisotropic one with kernel = stride per axis (e.g. (1, 2, 2)) runs on conv_gather_tc: one tap per parity class."""
+        s = tuple(int(i) for i in conv.stride)
+        if s != (2, 2, 2):
+            y, _ = K.conv_gather_tc(x, self._wg(conv, key, s, s, 0, transposed=True), cin, conv.out_channels, s, s, 0, transposed=True,
+                                    bias=conv.bias, out=out, out_coff=out_coff)
+            return y
         y, _ = K.gemm_tc(x, self._wup(conv, key), cin, 8 * conv.out_channels, bias=conv.bias, out=out, out_coff=out_coff, mode=2)
         return y
 

@@ -9,13 +9,18 @@ reference checkpoint loads key for key.  Inference only: deep-supervision heads 
 full-resolution output is produced, which is what the reference returns in eval mode.
 
 Two forwards, chosen from the input and the configuration (DESIGN.md §8.4):
-  * fp16 CUDA input and an eligible configuration (`_tc_ok`: 3-D, every kernel 3, strides [1, 2, 2, ...], upsample kernels equal
-    to the strides, filters % 16 == 0, InstanceNorm with or without affine and without running statistics, LeakyReLU with a
-    slope in [0, 1], out_channels <= 16; dropout inactive at call time): `_forward_tc`, the whole network on fp16 channel-blocked
-    (NC8) buffers and Hopper tensor cores -- `b200_conv3x3x3_tc` for the stride-1 3x3x3 convolutions (the previous norm +
-    LeakyReLU applied on the operand load), `b200_conv_gather_tc` for the stride-2 ones, `b200_gemm_tc` for the transposed
-    convolutions, the output head `b200_head_conv_norm_nc8` with the affine norm -- replayed from a CUDA graph per input shape;
-  * everything else (fp32 input, anisotropic plans, other norms): `_forward_generic`, the fp32-faithful generic kernels.
+  * fp16 CUDA input and an eligible configuration (`_tc_ok`: 3-D; every kernel 3x3x3 or 3x3 in one plane and 1 along the third
+    axis, e.g. [1, 3, 3]; strides[0] == 1 and every later stride 1 or 2 per axis with a 2 on at least one axis -- the isotropic
+    [1, 2, 2, ...] plans and the anisotropic nnU-Net plans such as [[1,1,1], [1,2,2], [1,2,2], [2,2,2], ...]; upsample kernels equal
+    to the strides per axis; filters % 16 == 0, InstanceNorm with or without affine and without running statistics, LeakyReLU with
+    a slope in [0, 1], out_channels <= 16; dropout inactive at call time): `_forward_tc`, the whole network on fp16 channel-blocked
+    (NC8) buffers and Hopper tensor cores -- `b200_conv3x3x3_tc` for the stride-1 3x3x3 convolutions and `b200_conv3x3_tc` for the
+    stride-1 one-plane ones (the previous norm + LeakyReLU applied on the operand load), `b200_conv_gather_tc` for the strided ones
+    (per axis), `b200_gemm_tc` for the (2, 2, 2) transposed convolutions and `b200_conv_gather_tc` for the anisotropic ones, the
+    output head `b200_head_conv_norm_nc8` with the affine norm -- replayed from a CUDA graph per input shape.  The input's spatial
+    sizes must be divisible, per axis, by the product of the strides;
+  * everything else (fp32 input, kernels with two axes of size 1 or of size 5, stride 3, other norms): `_forward_generic`, the
+    fp32-faithful generic kernels.
 """
 from __future__ import annotations
 
@@ -48,9 +53,9 @@ class DynUNetSkipLayer(nn.Module):
         return self.upsample(self.next_layer(down), down)   # supervision heads only matter in training mode
 
 
-def _all(v, want: int) -> bool:
-    """An int or a per-axis sequence that equals `want` on every axis."""
-    return all(int(i) == want for i in (v if isinstance(v, (list, tuple)) else [v]))
+def _t3(v) -> tuple[int, ...]:
+    """An int or a per-axis sequence as a per-axis tuple (3 axes; a sequence keeps its own length)."""
+    return tuple(int(i) for i in v) if isinstance(v, (list, tuple)) else (int(v),) * 3
 
 
 class DynUNet(TcNet, nn.Module):
@@ -126,13 +131,17 @@ class DynUNet(TcNet, nn.Module):
         self._tc_setup()
 
     def _tc_eligible(self) -> bool:
-        """Whether `_forward_tc` implements this configuration (isotropic 3x3x3 / stride-2 plans, InstanceNorm, LeakyReLU)."""
-        st, up = self.strides, self.upsample_kernel_size
+        """Whether `_forward_tc` implements this configuration (3x3x3 or one-plane 3x3 kernels, strides of 1 or 2 per axis,
+        InstanceNorm, LeakyReLU)."""
+        st, up = [_t3(s) for s in self.strides], [_t3(u) for u in self.upsample_kernel_size]
         if self.spatial_dims != 3 or self.out_channels > 16 or any(f % 16 for f in self.filters):
             return False
-        if not all(_all(k, 3) for k in self.kernel_size) or not _all(st[0], 1) or not all(_all(s, 2) for s in st[1:]):
+        one_plane = {(1, 3, 3), (3, 1, 3), (3, 3, 1)}
+        if not all(_t3(k) == (3, 3, 3) or _t3(k) in one_plane for k in self.kernel_size):
             return False
-        if len(up) != len(st) - 1 or not all(_all(u, 2) for u in up):
+        if st[0] != (1, 1, 1) or not all(set(s) <= {1, 2} and 2 in s for s in st[1:]):
+            return False
+        if len(up) != len(st) - 1 or any(u != s for u, s in zip(up, st[1:])):
             return False
         blocks = [self.input_block, *self.downsamples, self.bottleneck, *(u.conv_block for u in self.upsamples)]
         for b in blocks:
@@ -177,8 +186,23 @@ class DynUNet(TcNet, nn.Module):
         return self.output_block(self.skip_layers(x))
 
     # ------------------------------------------------------------------------------------------- tensor-core path
+    def _level_shapes(self, sp0: Sequence[int]) -> list[tuple[int, int, int]]:
+        """The spatial shape of every level: the input's divided by the cumulative strides, per axis."""
+        out, cur = [], (1, 1, 1)
+        for s in self.strides:
+            cur = tuple(c * i for c, i in zip(cur, _t3(s)))
+            out.append(tuple(int(v) // c for v, c in zip(sp0, cur)))
+        return out
+
     def _check_tc_input(self, x: torch.Tensor) -> None:
-        self._check_levels(x, len(self.strides))
+        if x.dim() != 5 or x.shape[1] != self.in_channels:
+            raise ValueError(f"DynUNet expects an [N, {self.in_channels}, D, H, W] input, got {tuple(x.shape)}")
+        div = [1, 1, 1]
+        for s in self.strides:
+            div = [d * i for d, i in zip(div, _t3(s))]
+        if any(int(v) % d for v, d in zip(x.shape[2:], div)):
+            raise ValueError(f"DynUNet with {len(self.strides)} levels needs spatial sizes divisible by {div[0]} x {div[1]} x {div[2]}, "
+                             f"got {tuple(x.shape[2:])}")
 
     def _forward_tc(self, x_in: torch.Tensor) -> torch.Tensor:
         """DynUNet.forward (dynunet.py:265-274, eval mode) on fp16 NC8 buffers and tensor cores; the output is fp16.
@@ -190,18 +214,19 @@ class DynUNet(TcNet, nn.Module):
             x_in = x_in.contiguous()
             n, dev, f = x_in.shape[0], x_in.device, self.filters
             nl = len(f)
-            sp0 = tuple(int(s) for s in x_in.shape[2:])
-            cats = [K.NC8(n, 2 * f[i], tuple(s >> i for s in sp0), dev) for i in range(nl - 1)]
+            shapes = self._level_shapes(x_in.shape[2:])
+            cats = [K.NC8(n, 2 * f[i], shapes[i], dev) for i in range(nl - 1)]
             block = self._res_block if self.conv_block is UnetResBlock else self._basic_block
 
-            if self.in_channels == 1:   # the raw NCDHW window feeds the single-channel stem kernels
+            if self.in_channels == 1 and self._one_plane_axis(self.input_block.conv1.conv) < 0:
+                # the raw NCDHW window feeds the single-channel 3x3x3 stem kernels
                 block(None, 1, 0, self.input_block, "in", out=cats[0], out_coff=f[0], x_in_raw=x_in)
             else:
                 xp, cp = self._pack_input(x_in)
                 block(xp, cp, 0, self.input_block, "in", out=cats[0], out_coff=f[0], cin_pad=cp)
             for j, down in enumerate(self.downsamples):
-                block(cats[j], f[j], f[j], down, f"d{j}", out=cats[j + 1], out_coff=f[j + 1], stride=2)
-            cur = block(cats[nl - 2], f[nl - 2], f[nl - 2], self.bottleneck, "bn", stride=2)
+                block(cats[j], f[j], f[j], down, f"d{j}", out=cats[j + 1], out_coff=f[j + 1])
+            cur = block(cats[nl - 2], f[nl - 2], f[nl - 2], self.bottleneck, "bn")
 
             for u, up in enumerate(self.upsamples):
                 lvl = nl - 2 - u

@@ -2,14 +2,19 @@
 """A network with a tensor-core forward as the predictor of a sliding-window inference, on deployed configurations:
 
   * unetr:               the reference's defaults (ViT-B/16, feature_size 16, 14 classes); a 256^3 fp16 volume, roi 96^3;
-  * dynunet:             the nnU-Net default plan (6 levels, filters 32 ... 320, affine instance norm, 14 classes); a 384^3 fp16
+  * dynunet iso:         the nnU-Net default plan (6 levels, filters 32 ... 320, affine instance norm, 14 classes); a 384^3 fp16
                          volume, roi 128^3;
+  * dynunet aniso_d:     an nnU-Net anisotropic plan for thick-slice CT / MR (kernels [1,3,3] at the two high-resolution levels,
+                         strides [1,2,2], [1,2,2], [2,2,2], [2,2,2], [1,2,2]; filters 32 ... 320, 14 classes); a 64 x 512 x 512 fp16
+                         volume, roi 32 x 256 x 256 (27 windows);
+  * dynunet aniso_w:     a MONAI-style plan with kernel 1 along W (kernels [3,3,1] at two levels, strides [2,2,1], [2,2,1], [2,2,2],
+                         [2,2,2]), residual blocks, filters 32 ... 320, 14 classes; a 384 x 384 x 64 fp16 volume, roi 192 x 192 x 32;
   * segresnet brats:     init_filters 16, 4 input modalities, 3 outputs, GroupNorm(8), blocks (1,2,2,4) / (1,1,1); a
                          4 x 240 x 240 x 160 fp16 volume, roi 128^3;
   * segresnet wholebody: init_filters 32, 1 input channel, 105 outputs, GroupNorm(8); a 256^3 fp16 volume, roi 96^3.
 
-    python scripts/sliding_window_tc.py --net unetr|dynunet|segresnet [--workload brats|wholebody|both] [--sw-batch 4]
-                                        [--steps 3] [--warmup 1]
+    python scripts/sliding_window_tc.py --net unetr|dynunet|segresnet [--workload brats|wholebody|both (SegResNet) |
+                                        iso|aniso_d|aniso_w|all (DynUNet)] [--sw-batch 4] [--steps 3] [--warmup 1]
 
 Overlap 0.5, gaussian blending.  Every batch shape (the full batches and the remainder batch) is warmed up first; each timed step
 is bracketed by CUDA events with a 256 MiB L2 flush before it (outside the timed interval), and the spread of the timed steps is
@@ -63,21 +68,31 @@ def unetr_flops(net, roi) -> dict:
     return {"vit": vit, "decoder": dec, "total": vit + dec}
 
 
+def _per_axis(v) -> tuple[int, int, int]:
+    return tuple(int(i) for i in v) if isinstance(v, (list, tuple)) else (int(v),) * 3
+
+
 def dynunet_flops(net, roi) -> dict:
-    """Multiply-add FLOPs (x2) of one window, from the layer shapes of DynUNet.forward (isotropic stride-2 plan)."""
+    """Multiply-add FLOPs (x2) of one window, from the layer shapes of DynUNet.forward: per-level kernel volumes and per-axis
+    strides (the isotropic plan: 3x3x3 kernels, stride 2)."""
     f, cin, nl = net.filters, net.in_channels, len(net.filters)
-    v = [math.prod(s // 2**k for s in roi) for k in range(nl)]   # voxels at level k
+    v, cum = [], (1, 1, 1)
+    for s in net.strides:                               # voxels at level k: the roi over the cumulative strides
+        cum = tuple(c * i for c, i in zip(cum, _per_axis(s)))
+        v.append(math.prod(r // c for r, c in zip(roi, cum)))
+    kv = [math.prod(_per_axis(k)) for k in net.kernel_size]   # kernel volume of level k
     res = net.conv_block.__name__ == "UnetResBlock"
 
-    def block(ci, co, n, skip_conv):   # two 3x3x3 convolutions (+ the 1x1x1 one of a residual block when shape or channels change)
-        return 2.0 * n * 27 * (ci * co + co * co) + (2.0 * n * ci * co if res and skip_conv else 0.0)
+    def block(ci, co, n, taps, skip_conv):   # two convolutions (+ the 1x1x1 one of a residual block when shape or channels change)
+        return 2.0 * n * taps * (ci * co + co * co) + (2.0 * n * ci * co if res and skip_conv else 0.0)
 
-    enc = block(cin, f[0], v[0], cin != f[0])
-    for k in range(1, nl):                              # down blocks and the bottleneck (stride 2: output voxels v[k])
-        enc += block(f[k - 1], f[k], v[k], True)
+    enc = block(cin, f[0], v[0], kv[0], cin != f[0])
+    for k in range(1, nl):                              # down blocks and the bottleneck (output voxels v[k])
+        enc += block(f[k - 1], f[k], v[k], kv[k], True)
     dec = 2.0 * v[0] * f[0] * net.out_channels
-    for k in range(nl - 2, -1, -1):                     # up blocks: ConvTranspose3d k2 s2, then a basic block on the concat
-        dec += 2.0 * v[k] * f[k + 1] * f[k] + 2.0 * v[k] * 27 * (2 * f[k] * f[k] + f[k] * f[k])
+    for k in range(nl - 2, -1, -1):                     # up blocks: ConvTranspose3d (kernel = stride: one tap per output voxel), then
+        # a basic block with the kernel of level k + 1 on the concat
+        dec += 2.0 * v[k] * f[k + 1] * f[k] + 2.0 * v[k] * kv[k + 1] * (2 * f[k] * f[k] + f[k] * f[k])
     return {"encoder": enc, "decoder": dec, "total": enc + dec}
 
 
@@ -118,6 +133,12 @@ def _nets():
                 make=lambda: DynUNet(3, 1, 14, kernel_size=[3] * 6, strides=[1, 2, 2, 2, 2, 2], upsample_kernel_size=[2] * 5), seed=30, cin=1,
                 volume=(384, 384, 384), roi=(128, 128, 128), flops=dynunet_flops,
                 desc="DynUNet(in=1, out=14, k=3x6, strides=[1,2,2,2,2,2], filters=32..320, affine IN)"),
+            "dynunet_sliding_window_aniso_d": dict(
+                make=lambda: DynUNet(3, 1, 14, **ANISO_D), seed=30, cin=1, volume=(64, 512, 512), roi=(32, 256, 256), flops=dynunet_flops,
+                desc="DynUNet(in=1, out=14, k=[1,3,3]x2 + 3x4, strides=[1,1,1],[1,2,2],[1,2,2],[2,2,2],[2,2,2],[1,2,2], filters=32..320, affine IN)"),
+            "dynunet_sliding_window_aniso_w": dict(
+                make=lambda: DynUNet(3, 1, 14, **ANISO_W), seed=30, cin=1, volume=(384, 384, 64), roi=(192, 192, 32), flops=dynunet_flops,
+                desc="DynUNet(in=1, out=14, k=[3,3,1]x2 + 3x3, strides=[1,1,1],[2,2,1],[2,2,1],[2,2,2],[2,2,2], res blocks, filters=32..320, affine IN)"),
         },
         "segresnet": {
             "segresnet_sliding_window_brats": dict(
@@ -130,6 +151,15 @@ def _nets():
                 desc="SegResNet(init=32, in=1, out=105, GroupNorm(8), blocks (1, 2, 2, 4)/(1, 1, 1), nontrainable)"),
         },
     }
+
+
+# the anisotropic DynUNet plans of the aniso_d / aniso_w workloads (the shapes of tests/golden/dynunet_aniso_cases.py A and B)
+ANISO_D = dict(kernel_size=[[1, 3, 3], [1, 3, 3], [3, 3, 3], [3, 3, 3], [3, 3, 3], [3, 3, 3]],
+               strides=[[1, 1, 1], [1, 2, 2], [1, 2, 2], [2, 2, 2], [2, 2, 2], [1, 2, 2]],
+               upsample_kernel_size=[[1, 2, 2], [1, 2, 2], [2, 2, 2], [2, 2, 2], [1, 2, 2]])
+ANISO_W = dict(kernel_size=[[3, 3, 1], [3, 3, 1], [3, 3, 3], [3, 3, 3], [3, 3, 3]], strides=[[1, 1, 1], [2, 2, 1], [2, 2, 1], [2, 2, 2], [2, 2, 2]],
+               upsample_kernel_size=[[2, 2, 1], [2, 2, 1], [2, 2, 2], [2, 2, 2]], filters=[32, 64, 128, 256, 320], res_block=True)
+DYNUNET_WORKLOADS = {"iso": "dynunet_sliding_window", "aniso_d": "dynunet_sliding_window_aniso_d", "aniso_w": "dynunet_sliding_window_aniso_w"}
 
 
 def _card() -> dict:
@@ -233,7 +263,8 @@ def run(metric: str, wl: dict, args, card: dict) -> dict:
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--net", required=True, choices=["unetr", "dynunet", "segresnet"])
-    ap.add_argument("--workload", default="both", choices=["both", "brats", "wholebody"], help="SegResNet only")
+    ap.add_argument("--workload", default=None, choices=["both", "brats", "wholebody", "all", "iso", "aniso_d", "aniso_w"],
+                    help="SegResNet: brats|wholebody|both (default both); DynUNet: iso|aniso_d|aniso_w|all (default iso)")
     ap.add_argument("--sw-batch", type=int, default=4)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
@@ -242,8 +273,11 @@ def main() -> None:
     if not torch.cuda.is_available():
         raise SystemExit("sliding_window_tc.py measures on a CUDA device; none is available")
     workloads = _nets()[args.net]
-    if args.net == "segresnet" and args.workload != "both":
+    if args.net == "segresnet" and args.workload not in (None, "both"):
         workloads = {f"segresnet_sliding_window_{args.workload}": workloads[f"segresnet_sliding_window_{args.workload}"]}
+    if args.net == "dynunet" and args.workload != "all":
+        name = DYNUNET_WORKLOADS[args.workload or "iso"]
+        workloads = {name: workloads[name]}
     card = _card()
     for metric, wl in workloads.items():
         print(json.dumps(run(metric, wl, args, card)), flush=True)
