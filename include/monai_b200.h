@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 4
+#define B200_ABI_VERSION 5
 
 /* ---- library ---------------------------------------------------------------------------------------- */
 int b200_abi_version(void);
@@ -416,14 +416,17 @@ int b200_head_conv_norm_nc8(const void* x, int N, int C, long long S, const floa
                             const float* bias, int Cout, void* y, int out_dtype, const float* gamma, const float* beta,
                             void* stream);
 
-/* NC8 variant of b200_norm_act: y = act(instnorm(x) * gamma + beta [+ instnorm?(res) * res_gamma + res_beta]); act: 0 none,
- * 1 leaky-relu(slope), 3 relu.  x / res / y are channel slices [coff, coff+C) of NC8 buffers with ctot channels.  The affine
- * parameters (UnetResBlock norm2 and norm3 with affine=True, dynunet_block.py:97-111) are float32 device [C] or NULL (1 / 0);
- * gamma / beta need stats, res_gamma / res_beta need res_stats. */
+/* NC8 variant of b200_norm_act; act: 0 none, 1 leaky-relu(slope), 3 relu.  res_mode chooses where res is added (ABI 5):
+ *   0: y = act(instnorm(x) * gamma + beta [+ instnorm?(res) * res_gamma + res_beta])   (UnetResBlock, dynunet_block.py:97-111)
+ *   1: y = act(instnorm(x) * gamma + beta) + res                                       (ResidualUnit, convolutions.py:156-161)
+ * x / res / y are channel slices [coff, coff+C) of NC8 buffers with ctot channels.  stats == NULL skips the normalisation (the
+ * activation alone, e.g. after a convolution with an eval-mode BatchNorm folded into its weights).  The affine parameters are
+ * float32 device [C] or NULL (1 / 0); gamma / beta need stats, res_gamma / res_beta need res_stats.  Mode 1 adds res as it is:
+ * res_stats, res_gamma and res_beta must be NULL (B200_ERR_INVALID otherwise). */
 int b200_norm_act_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats, float eps,
                       const void* res, int res_ctot, int res_coff, const float* res_stats, int act, float slope,
                       void* y, int y_ctot, int y_coff, const float* gamma, const float* beta, const float* res_gamma,
-                      const float* res_beta, void* stream);
+                      const float* res_beta, int res_mode, void* stream);
 
 /* GroupNorm statistics from per-channel ones (nn.GroupNorm, SegResNet's default norm): stats = {sum, sumsq} per (n, channel)
  * [N][C][2] as written by the `stats` outputs of these entry points; for channel c of group g (cpg = C / groups channels each)

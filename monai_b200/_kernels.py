@@ -668,16 +668,17 @@ def norm_act_nc8(
     x: NC8, C_: int, stats: torch.Tensor | None, x_coff: int = 0, res: NC8 | None = None, res_coff: int = 0,
     res_stats: torch.Tensor | None = None, act: int = L.ACT_NONE, slope: float = 0.0, out: NC8 | None = None,
     out_coff: int = 0, eps: float = 1e-5, gamma: torch.Tensor | None = None, beta: torch.Tensor | None = None,
-    res_gamma: torch.Tensor | None = None, res_beta: torch.Tensor | None = None,
+    res_gamma: torch.Tensor | None = None, res_beta: torch.Tensor | None = None, res_after_act: bool = False,
 ) -> NC8:
     """y = act(instnorm(x) [+ instnorm?(res)]) on NC8 channel slices; gamma / beta (res_gamma / res_beta) are the affine
-    parameters of x's (res's) InstanceNorm."""
+    parameters of x's (res's) InstanceNorm.  `res_after_act`: y = act(instnorm(x)) + res instead (ResidualUnit's `cx + res`),
+    with res added as it is (no res_stats / res_gamma / res_beta).  stats None: no normalisation, the activation alone."""
     if out is None:
         out = NC8(x.N, C_, x.sp, x.buf.device)
     affine = [_f32c(t) for t in (gamma, beta, res_gamma, res_beta)]
     _call("norm_act_nc8", L.ptr(x.buf), x.C, x_coff, x.N, C_, x.S, L.ptr(stats), eps, L.ptr(res.buf) if res is not None else None,
           res.C if res is not None else 0, res_coff, L.ptr(res_stats), act, float(slope), L.ptr(out.buf), out.C, out_coff,
-          *map(L.ptr, affine), L.stream_ptr(x.buf.device),
+          *map(L.ptr, affine), int(bool(res_after_act)), L.stream_ptr(x.buf.device),
           label="norm_act_affine_nc8" if any(t is not None for t in affine) else "norm_act_nc8")
     return out
 

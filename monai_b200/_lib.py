@@ -14,7 +14,7 @@ import torch
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = _HERE / "lib" / "libmonai_b200.so"
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 DT_F32, DT_F16 = 0, 1
 _DT = {torch.float32: DT_F32, torch.float16: DT_F16}
 
@@ -131,7 +131,7 @@ SIGNATURES = {
     "b200_channel_post": (i32, [vp, i32, i32, i64, i32, f32, i32, vp, i32, vp]),
     "b200_head_conv_nc8": (i32, [vp, i32, i32, i64, vp, vp, i32, vp, i32, vp]),
     "b200_head_conv_norm_nc8": (i32, [vp, i32, i32, i64, vp, f32, vp, i32, i32, vp, f32, vp, vp, i32, vp, i32, vp, vp, vp]),
-    "b200_norm_act_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, i32, i32, vp, i32, f32, vp, i32, i32, vp, vp, vp, vp, vp]),
+    "b200_norm_act_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, i32, i32, vp, i32, f32, vp, i32, i32, vp, vp, vp, vp, i32, vp]),
     "b200_norm_act_cin1res_nc8": (i32, [vp, i32, i32, i32, i32, i64, vp, f32, vp, vp, vp, i32, f32, vp, i32, i32, vp]),
     "b200_group_stats": (i32, [vp, i32, i32, i32, vp, vp]),
     "b200_upsample_add_nc8_workspace_bytes": (i64, [i32] * 6),

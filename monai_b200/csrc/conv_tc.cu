@@ -466,8 +466,9 @@ struct NormActNc8P {
 // instantiation then compiles to the code (and the 48 registers) it had before the affine variant existed.
 struct NormAffineP { const float* gamma; const float* beta; const float* res_gamma; const float* res_beta; };
 
-// AFFINE: apply the affine parameters `a` (a separate instantiation, so the non-affine launches keep their registers)
-template <bool AFFINE>
+// AFFINE: apply the affine parameters `a` (a separate instantiation, so the non-affine launches keep their registers).
+// POST: add res as it is after the activation, act(norm(x)) + res (ResidualUnit); res_stats and raw are NULL then
+template <bool AFFINE, bool POST = false>
 __global__ void __launch_bounds__(256) norm_act_nc8_kernel(NormActNc8P p, NormAffineP a) {
   const int chunk = blockIdx.y, n = blockIdx.z;
   float sc[8], sh[8], rsc[8], rsh[8];
@@ -505,10 +506,15 @@ __global__ void __launch_bounds__(256) norm_act_nc8_kernel(NormActNc8P p, NormAf
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       float f = fmaf(__half2float(v[j]), sc[j], sh[j]);
-      if (r) f += fmaf(__half2float(rv[j]), rsc[j], rsh[j]);
-      if (u) f += fmaf(uv, rsc[j], rsh[j]);
+      if constexpr (!POST) {
+        if (r) f += fmaf(__half2float(rv[j]), rsc[j], rsh[j]);
+        if (u) f += fmaf(uv, rsc[j], rsh[j]);
+      }
       if (p.act == 1) f = f >= 0.f ? f : f * p.slope;
       else if (p.act == 3) f = fmaxf(f, 0.f);
+      if constexpr (POST) {
+        if (r) f += __half2float(rv[j]);
+      }
       v[j] = __float2half_rn(f);
     }
     *reinterpret_cast<uint4*>(y + s * 8) = *reinterpret_cast<const uint4*>(v);
@@ -763,11 +769,13 @@ extern "C" int b200_conv3x3_tc(const b200_conv_tc_desc* desc, int axis, const vo
 }
 
 // sizes the grid and launches norm_act_nc8_kernel: the body of b200_norm_act_nc8 and b200_norm_act_cin1res_nc8
-static int norm_act_nc8_launch(const NormActNc8P& p, int N, const NormAffineP& a, void* stream) {
+static int norm_act_nc8_launch(const NormActNc8P& p, int N, const NormAffineP& a, void* stream, bool post = false) {
   if ((long long)N * p.C * p.S == 0) return B200_OK;
   long long want = (long long)num_sms() * 16 / ((long long)N * (p.C / 8)) + 1;
   dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(want, (p.S + 255) / 256)), p.C / 8, N);
-  if (a.gamma || a.beta || a.res_gamma || a.res_beta) norm_act_nc8_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
+  if (post && (a.gamma || a.beta)) norm_act_nc8_kernel<true, true><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
+  else if (post) norm_act_nc8_kernel<false, true><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
+  else if (a.gamma || a.beta || a.res_gamma || a.res_beta) norm_act_nc8_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
   else norm_act_nc8_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(p, a);
   B200_LAUNCH_CHECK("norm_act_nc8_kernel");
   return B200_OK;
@@ -776,15 +784,17 @@ static int norm_act_nc8_launch(const NormActNc8P& p, int N, const NormAffineP& a
 extern "C" int b200_norm_act_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats,
                                  float eps, const void* res, int res_ctot, int res_coff, const float* res_stats, int act,
                                  float slope, void* y, int y_ctot, int y_coff, const float* gamma, const float* beta,
-                                 const float* res_gamma, const float* res_beta, void* stream) {
+                                 const float* res_gamma, const float* res_beta, int res_mode, void* stream) {
   B200_REQUIRE(x && y, "norm_act_nc8: null pointer");
+  B200_REQUIRE(res_mode == 0 || res_mode == 1, "norm_act_nc8: res_mode must be 0 (add before the activation) or 1 (after it)");
+  B200_REQUIRE(res_mode == 0 || !(res_stats || res_gamma || res_beta), "norm_act_nc8: res_mode 1 adds res as it is (no res_stats, res_gamma, res_beta)");
   B200_REQUIRE(C % 8 == 0 && x_ctot % 8 == 0 && x_coff % 8 == 0 && y_ctot % 8 == 0 && y_coff % 8 == 0, "norm_act_nc8: channels must be multiples of 8");
   B200_REQUIRE(act == 0 || act == 1 || act == 3, "norm_act_nc8: activation must be none, leaky-relu or relu");
   B200_REQUIRE(stats || !(gamma || beta), "norm_act_nc8: affine parameters without statistics");
   B200_REQUIRE(res_stats || !(res_gamma || res_beta), "norm_act_nc8: residual affine parameters without residual statistics");
   const NormActNc8P p{(const __half*)x, (__half*)y, (const __half*)res, C, x_ctot, x_coff, y_ctot, y_coff, res_ctot, res_coff, S,
                       stats, res_stats, eps, act, slope, nullptr, nullptr, nullptr};
-  return norm_act_nc8_launch(p, N, NormAffineP{gamma, beta, res_gamma, res_beta}, stream);
+  return norm_act_nc8_launch(p, N, NormAffineP{gamma, beta, res_gamma, res_beta}, stream, res_mode == 1);
 }
 
 extern "C" int b200_norm_act_cin1res_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats,

@@ -6,7 +6,7 @@ It owns what those networks share:
   * CUDA-graph replay of `_forward_tc`.  One forward is tens to hundreds of short kernel launches; issuing them from Python
     through ctypes costs more than the kernels themselves once they are fast, so the launch sequence for a given input shape is
     captured once into a CUDA graph and replayed.  Graphs are keyed by (shape, dtype, device) and invalidated when any parameter
-    changes (`load_state_dict`, `.half()`).  MONAI_B200_GRAPH=0 disables the mechanism;
+    or buffer changes (`load_state_dict`, `.half()`).  MONAI_B200_GRAPH=0 disables the mechanism;
   * the packed-weight cache, the channel-padded input stem, and the residual / basic blocks, transposed convolutions and output
     head of the CNN parts.  The block helpers accept any module with the `conv1.conv` / `conv2.conv` / optional `conv3.conv`,
     `norm1/2/3` and `lrelu` structure of UnetResBlock / UnetBasicBlock (dynunet_block.py:25-177; InstanceNorm with or without affine
@@ -85,7 +85,8 @@ class TcNet:
         return self._graph_enabled and not K._Prof.on and not torch.cuda.is_current_stream_capturing()
 
     def _forward_graphed(self, x_in: torch.Tensor) -> torch.Tensor:
-        sig = tuple((p.data_ptr(), p._version) for p in self.parameters())
+        # buffers too: load_state_dict may change only a BatchNorm's running statistics, which a folded weight depends on
+        sig = tuple((p.data_ptr(), p._version) for p in (*self.parameters(), *self.buffers()))
         key = (tuple(x_in.shape), x_in.dtype, x_in.device)
         ent = self._graphs.get(key)
         if ent is None or ent["sig"] != sig:

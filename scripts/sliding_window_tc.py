@@ -11,17 +11,22 @@
                          [2,2,2]), residual blocks, filters 32 ... 320, 14 classes; a 384 x 384 x 64 fp16 volume, roi 192 x 192 x 32;
   * segresnet brats:     init_filters 16, 4 input modalities, 3 outputs, GroupNorm(8), blocks (1,2,2,4) / (1,1,1); a
                          4 x 240 x 240 x 160 fp16 volume, roi 128^3;
-  * segresnet wholebody: init_filters 32, 1 input channel, 105 outputs, GroupNorm(8); a 256^3 fp16 volume, roi 96^3.
+  * segresnet wholebody: init_filters 32, 1 input channel, 105 outputs, GroupNorm(8); a 256^3 fp16 volume, roi 96^3;
+  * unet res_batch:      the spleen CT UNet of MONAI's tutorial and bundle (channels 16 ... 256, strides 2, two residual units,
+                         eval-mode BatchNorm, PReLU, 1 -> 2 channels); a 256^3 fp16 volume, roi 160^3;
+  * unet res_instance:   the same net with InstanceNorm (MONAI's default norm); a 256^3 fp16 volume, roi 96^3.
 
-    python scripts/sliding_window_tc.py --net unetr|dynunet|segresnet [--workload brats|wholebody|both (SegResNet) |
-                                        iso|aniso_d|aniso_w|all (DynUNet)] [--sw-batch 4] [--steps 3] [--warmup 1]
+    python scripts/sliding_window_tc.py --net unetr|dynunet|segresnet|unet [--workload brats|wholebody|both (SegResNet) |
+                                        iso|aniso_d|aniso_w|all (DynUNet) | res_batch|res_instance|res (UNet)] [--sw-batch 4]
+                                        [--steps 3] [--warmup 1]
 
 Overlap 0.5, gaussian blending.  Every batch shape (the full batches and the remainder batch) is warmed up first; each timed step
 is bracketed by CUDA events with a 256 MiB L2 flush before it (outside the timed interval), and the spread of the timed steps is
 reported.  A separate profiled step lists device time per kernel.  Finally one forward of sw_batch windows and one of a single
 window are timed on each path: `net(x)` (tensor cores) and `net._forward_generic(x)` (the generic CUDA-core kernels), giving the
-speed-up per window without running a whole volume on CUDA cores.  Prints one JSON line per workload, with the card name and
-power limit read in the same run.
+speed-up per window without running a whole volume on CUDA cores; for UNet the tensor-core forward is also timed per window eager
+(without CUDA-graph replay), and with BatchNorm the activation-only norm_act_nc8 passes of one forward are timed on their own.
+Prints one JSON line per workload, with the card name and power limit read in the same run.
 """
 from __future__ import annotations
 
@@ -119,8 +124,64 @@ def segresnet_flops(net, roi) -> dict:
     return {"encoder": enc, "decoder": dec, "total": enc + dec}
 
 
+def unet_flops(net, roi) -> dict:
+    """Multiply-add FLOPs (x2) of one window, from the layer shapes of UNet with residual units: every convolution of the down
+    ResidualUnits and the bottom one (encoder), and the transposed convolutions and up ResidualUnits (decoder)."""
+    import torch.nn as nn
+
+    from monai_b200.networks.blocks.convolutions import ResidualUnit
+
+    def conv(m, v):                      # (FLOPs, output voxels) of a Conv3d / ConvTranspose3d on v input voxels
+        k, s = math.prod(m.kernel_size), math.prod(m.stride)
+        if isinstance(m, nn.ConvTranspose3d):
+            return 2.0 * v * m.in_channels * m.out_channels * k, v * s
+        return 2.0 * (v // s) * m.in_channels * m.out_channels * k, v // s
+
+    def unit(mod, v):                    # a ResidualUnit or a Convolution block
+        if not isinstance(mod, ResidualUnit):
+            return conv(mod.conv, v)
+        f, vo = 0.0, v
+        for u in mod.conv:
+            fu, vo = conv(u.conv, vo)
+            f += fu
+        if not isinstance(mod.residual, nn.Identity):
+            f += conv(mod.residual, v)[0]
+        return f, vo
+
+    def level(block, v):                 # (encoder, decoder) FLOPs of Sequential(down, SkipConnection(sub), up)
+        down, sub, up = block[0], block[1].submodule, block[2]
+        enc, vd = unit(down, v)
+        if isinstance(sub, ResidualUnit):
+            e2, d2 = unit(sub, vd)[0], 0.0
+        else:
+            e2, d2 = level(sub, vd)
+        dec, vu = 0.0, vd
+        for m in (up if isinstance(up, nn.Sequential) else [up]):
+            f, vu = unit(m, vu)
+            dec += f
+        return enc + e2, d2 + dec
+
+    enc, dec = level(net.model, math.prod(roi))
+    return {"encoder": enc, "decoder": dec, "total": enc + dec}
+
+
+def unet_act_passes(net, roi, batch) -> list:
+    """(channels, spatial size) of each activation-only norm_act_nc8 pass of a BatchNorm residual UNet forward: the output of every
+    unit of a down or bottom ResidualUnit but its last, activated before the next unit's convolution reads it."""
+    from monai_b200.networks.blocks.convolutions import ResidualUnit
+
+    out, block, sp = [], net.model, tuple(roi)
+    while True:
+        down, sub = block[0], block[1].submodule
+        sp = tuple(v // down.conv.unit0.conv.stride[0] for v in sp)
+        out += [(down.out_channels, sp)] * (len(down.conv) - 1)
+        if isinstance(sub, ResidualUnit):
+            return out + [(sub.out_channels, sp)] * (len(sub.conv) - 1)
+        block = sub
+
+
 def _nets():
-    from monai_b200.networks.nets import UNETR, DynUNet, SegResNet
+    from monai_b200.networks.nets import UNETR, DynUNet, SegResNet, UNet
 
     return {
         "unetr": {
@@ -149,6 +210,16 @@ def _nets():
                 make=lambda: SegResNet(spatial_dims=3, init_filters=32, in_channels=1, out_channels=105, norm=("GROUP", {"num_groups": 8})),
                 seed=30, cin=1, volume=(256, 256, 256), roi=(96, 96, 96), flops=segresnet_flops,
                 desc="SegResNet(init=32, in=1, out=105, GroupNorm(8), blocks (1, 2, 2, 4)/(1, 1, 1), nontrainable)"),
+        },
+        "unet": {
+            "unet_sliding_window_res_batch": dict(
+                make=lambda: UNet(3, 1, 2, (16, 32, 64, 128, 256), (2, 2, 2, 2), num_res_units=2, norm="batch"), seed=20, cin=1,
+                volume=(256, 256, 256), roi=(160, 160, 160), flops=unet_flops, eager_vs_replay=True, act_passes=unet_act_passes,
+                desc="UNet(in=1, out=2, channels 16..256, strides 2, num_res_units=2, BatchNorm (eval), PReLU)"),
+            "unet_sliding_window_res_instance": dict(
+                make=lambda: UNet(3, 1, 2, (16, 32, 64, 128, 256), (2, 2, 2, 2), num_res_units=2), seed=20, cin=1,
+                volume=(256, 256, 256), roi=(96, 96, 96), flops=unet_flops, eager_vs_replay=True,
+                desc="UNet(in=1, out=2, channels 16..256, strides 2, num_res_units=2, InstanceNorm, PReLU)"),
         },
     }
 
@@ -200,7 +271,7 @@ def run(metric: str, wl: dict, args, card: dict) -> dict:
     net = wl["make"]()
     net.load_state_dict(fill_state_dict(net.state_dict(), wl["seed"]))
     net = net.half().eval().to(dev)
-    assert net._tc_ok
+    assert net._tc_eligible() if hasattr(net, "_tc_eligible") else net._tc_ok
     vol = torch.randn((1, cin, *volume), generator=torch.Generator().manual_seed(0)).half().to(dev)
     windows = _windows(volume, roi)
 
@@ -238,6 +309,23 @@ def run(metric: str, wl: dict, args, card: dict) -> dict:
             net._forward_generic(xb)   # loads the generic kernels
             gen_ms = _timed(net._forward_generic, xb, 1)
             per_window[f"batch{b}"] = {"tensor_core": round(tc_ms / b, 3), "generic": round(gen_ms / b, 3), "speedup": round(gen_ms / tc_ms, 1)}
+            if wl.get("eager_vs_replay"):   # the tensor-core forward once more with the other launch mode (CUDA-graph replay or eager)
+                graph = net._graph_enabled
+                net._graph_enabled = not graph
+                net(xb)
+                per_window[f"batch{b}"]["tensor_core_eager" if graph else "tensor_core_graph_replay"] = round(_timed(net, xb, 5) / b, 3)
+                net._graph_enabled = graph
+                net._graphs.clear()
+        if wl.get("act_passes"):
+            # the activation-only norm_act_nc8 passes that eval-mode BatchNorm adds (its units have no statistics to apply on the
+            # next convolution's operand load), each timed over 20 launches at the step's batch
+            passes = wl["act_passes"](net, roi, args.sw_batch)
+            x8 = {sh: K.NC8(args.sw_batch, sh[0], sh[1], dev) for sh in set(passes)}
+            for t in x8.values():
+                t.buf.normal_()
+            act_ms = sum(_timed(lambda t: K.norm_act_nc8(t, t.C, None, act=K.L.ACT_LEAKY, slope=0.25), x8[sh], 20) for sh in passes)
+            per_window["bn_act_passes"] = {"n_per_forward": len(passes), "ms_per_forward": round(act_ms, 3),
+                                           "ms_per_step": round(act_ms * -(-windows // args.sw_batch), 2)}
 
     fl = wl["flops"](net, roi)
     ms = sorted(times)[len(times) // 2]
@@ -262,9 +350,11 @@ def run(metric: str, wl: dict, args, card: dict) -> dict:
 
 def main() -> None:
     ap = argparse.ArgumentParser()
-    ap.add_argument("--net", required=True, choices=["unetr", "dynunet", "segresnet"])
-    ap.add_argument("--workload", default=None, choices=["both", "brats", "wholebody", "all", "iso", "aniso_d", "aniso_w"],
-                    help="SegResNet: brats|wholebody|both (default both); DynUNet: iso|aniso_d|aniso_w|all (default iso)")
+    ap.add_argument("--net", required=True, choices=["unetr", "dynunet", "segresnet", "unet"])
+    ap.add_argument("--workload", default=None, choices=["both", "brats", "wholebody", "all", "iso", "aniso_d", "aniso_w", "res_batch",
+                                                          "res_instance", "res"],
+                    help="SegResNet: brats|wholebody|both (default both); DynUNet: iso|aniso_d|aniso_w|all (default iso); "
+                         "UNet: res_batch|res_instance|res (default res: both)")
     ap.add_argument("--sw-batch", type=int, default=4)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
@@ -278,6 +368,8 @@ def main() -> None:
     if args.net == "dynunet" and args.workload != "all":
         name = DYNUNET_WORKLOADS[args.workload or "iso"]
         workloads = {name: workloads[name]}
+    if args.net == "unet" and args.workload not in (None, "res"):
+        workloads = {f"unet_sliding_window_{args.workload}": workloads[f"unet_sliding_window_{args.workload}"]}
     card = _card()
     for metric, wl in workloads.items():
         print(json.dumps(run(metric, wl, args, card)), flush=True)
