@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 5
+#define B200_ABI_VERSION 6
 
 /* ---- library ---------------------------------------------------------------------------------------- */
 int b200_abi_version(void);
@@ -453,6 +453,13 @@ int b200_upsample_add_nc8(const void* x, int x_ctot, int x_coff, int N, int C, i
 int b200_norm_act_cin1res_nc8(const void* x, int x_ctot, int x_coff, int N, int C, long long S, const float* stats, float eps,
                               const void* raw, const float* raw_stats, const float* raw_weight, int act, float slope, void* y,
                               int y_ctot, int y_coff, void* stream);
+
+/* y = 2x max pool of x on NC8 fp16 channel slices (ABI 6; BasicUNet's Down, basic_unet.py: nn.MaxPool3d(2)): x is channels
+ * [x_coff, x_coff + C) of a buffer with x_ctot channels at (D, H, W), y channels [y_coff, y_coff + C) of one with y_ctot channels at
+ * (D/2, H/2, W/2), rounded down as nn.MaxPool3d(2) rounds.  A NaN in a 2x2x2 cell gives NaN, as in torch.  C, x_coff and y_coff
+ * must be multiples of 8 and each slice must fit in its buffer (B200_ERR_INVALID otherwise).  y may not overlap x. */
+int b200_maxpool2_nc8(const void* x, int x_ctot, int x_coff, int N, int C, int D, int H, int W, void* y, int y_ctot, int y_coff,
+                      void* stream);
 
 #ifdef __cplusplus
 }

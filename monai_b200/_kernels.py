@@ -714,6 +714,19 @@ def upsample_add_nc8(x: NC8, C_: int, scale: int, skip: NC8, x_coff: int = 0, sk
     return out, stats
 
 
+def maxpool2_nc8(x: NC8, C_: int, x_coff: int = 0, out: NC8 | None = None, out_coff: int = 0) -> NC8:
+    """nn.MaxPool3d(2) of channels [x_coff, x_coff + C_) of x into channels [out_coff, out_coff + C_) of `out` (a new C_-channel image
+    when None) at half x's spatial size, rounded down; a NaN in a 2x2x2 cell gives NaN."""
+    sp = tuple(s // 2 for s in x.sp)
+    if out is None:
+        out = NC8(x.N, C_, sp, x.buf.device)
+    if out.N != x.N or out.sp != sp:
+        raise ValueError(f"maxpool2_nc8: output is {(out.N, *out.sp)}, expected {(x.N, *sp)}")
+    _call("maxpool2_nc8", L.ptr(x.buf), x.C, x_coff, x.N, C_, *x.sp, L.ptr(out.buf), out.C, out_coff, L.stream_ptr(x.buf.device),
+          nbytes=float(x.N * C_ * (8 * out.S + out.S) * 2))
+    return out
+
+
 def cat_channels(tensors: Sequence[torch.Tensor]) -> torch.Tensor:
     """torch.cat(tensors, dim=1) for [N,C_i,*spatial] tensors of one dtype, done by the channel-copy kernel."""
     t0 = tensors[0]

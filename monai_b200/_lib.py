@@ -14,7 +14,7 @@ import torch
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = _HERE / "lib" / "libmonai_b200.so"
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 DT_F32, DT_F16 = 0, 1
 _DT = {torch.float32: DT_F32, torch.float16: DT_F16}
 
@@ -136,6 +136,7 @@ SIGNATURES = {
     "b200_group_stats": (i32, [vp, i32, i32, i32, vp, vp]),
     "b200_upsample_add_nc8_workspace_bytes": (i64, [i32] * 6),
     "b200_upsample_add_nc8": (i32, [vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, i32, i32, vp, i32, i32, vp, vp, vp]),
+    "b200_maxpool2_nc8": (i32, [vp, i32, i32, i32, i32, i32, i32, i32, vp, i32, i32, vp]),
 }
 
 _lib = None

@@ -11,6 +11,9 @@
 // Statistics (stats.cuh): one block per (batch item, 8-channel chunk, slice of voxels); a thread walks a fixed strided subset of the
 // voxels, the block combines its threads in a fixed order and writes one partial row, and launch_stats_finish adds the rows in fp64.
 // No floating-point atomics: the sums are the same bits on every run.
+//
+// Also here: the 2x max pool of BasicUNet's encoder (basic_unet.py Down: nn.MaxPool3d(2)) on NC8 channel slices.  One thread per
+// (output voxel, 8-channel chunk) makes eight 16-byte loads and one 16-byte store; like the decoder join it is bound by HBM.
 #include "common.cuh"
 #include "stats.cuh"
 #include "../../include/monai_b200.h"
@@ -107,16 +110,62 @@ __global__ void __launch_bounds__(256) upsample_add_nc8_kernel(UpAddP p) {
   }
 }
 
-// blocks per (batch item, chunk): enough for eight 256-thread blocks per SM in all, never more than the voxels need
+// blocks per (batch item, chunk): enough for eight 256-thread blocks per SM in all, never more than the voxels need (also sizes
+// the max pool's grid)
 static int upsample_add_blocks(int N, int C, long long So) {
   const long long planes = (long long)N * (C / 8);
   const long long want = ((long long)num_sms() * 8 + planes - 1) / planes;
   return (int)std::max<long long>(1, std::min<long long>(want, (So + 255) / 256));
 }
 
+// y = max over the 2x2x2 cell of x, per channel; __hmax2_nan keeps a NaN, as torch's max pooling does
+__global__ void __launch_bounds__(256) maxpool2_nc8_kernel(const __half* __restrict__ x, int x_ctot, int x_coff, __half* __restrict__ y,
+                                                           int y_ctot, int y_coff, int D, int H, int W) {
+  const int chunk = blockIdx.y, n = blockIdx.z;
+  const int Do = D >> 1, Ho = H >> 1, Wo = W >> 1;
+  const long long Si = (long long)D * H * W, So = (long long)Do * Ho * Wo;
+  const __half* xs = x + (((long long)n * (x_ctot / 8) + x_coff / 8 + chunk) * Si) * 8;
+  __half* ys = y + (((long long)n * (y_ctot / 8) + y_coff / 8 + chunk) * So) * 8;
+  for (long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x; s < So; s += (long long)gridDim.x * blockDim.x) {
+    const int ow = (int)(s % Wo);
+    const long long t = s / Wo;
+    const int oh = (int)(t % Ho), od = (int)(t / Ho);
+    const __half* p = xs + (((long long)(2 * od) * H + 2 * oh) * W + 2 * ow) * 8;
+    uint4 m = __ldg(reinterpret_cast<const uint4*>(p));
+    __half2* mh = reinterpret_cast<__half2*>(&m);
+#pragma unroll
+    for (int k = 1; k < 8; ++k) {
+      const long long off = ((long long)((k >> 2) & 1) * H * W + (long long)((k >> 1) & 1) * W + (k & 1)) * 8;
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(p + off));
+      const __half2* vh = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) mh[j] = __hmax2_nan(mh[j], vh[j]);
+    }
+    *reinterpret_cast<uint4*>(ys + s * 8) = m;
+  }
+}
+
 }  // namespace b200
 
 using namespace b200;
+
+extern "C" int b200_maxpool2_nc8(const void* x, int x_ctot, int x_coff, int N, int C, int D, int H, int W, void* y, int y_ctot, int y_coff,
+                                 void* stream) {
+  B200_REQUIRE(x && y, "maxpool2_nc8: null pointer");
+  B200_REQUIRE(N > 0 && C > 0 && D > 0 && H > 0 && W > 0, "maxpool2_nc8: empty problem");
+  B200_REQUIRE(C % 8 == 0 && x_ctot % 8 == 0 && x_coff % 8 == 0 && x_coff >= 0 && x_coff + C <= x_ctot,
+               "maxpool2_nc8: bad channel slice of x (C %d, x_coff %d, x_ctot %d)", C, x_coff, x_ctot);
+  B200_REQUIRE(y_ctot % 8 == 0 && y_coff % 8 == 0 && y_coff >= 0 && y_coff + C <= y_ctot,
+               "maxpool2_nc8: bad channel slice of y (C %d, y_coff %d, y_ctot %d)", C, y_coff, y_ctot);
+  B200_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0, "maxpool2_nc8: pointers must be 16-byte aligned");
+  B200_REQUIRE(C / 8 <= 65535 && N <= 65535, "maxpool2_nc8: N or C too large for one launch");
+  const long long So = (long long)(D / 2) * (H / 2) * (W / 2);
+  if (So == 0) return B200_OK;
+  dim3 grid(upsample_add_blocks(N, C, So), C / 8, N);
+  maxpool2_nc8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const __half*)x, x_ctot, x_coff, (__half*)y, y_ctot, y_coff, D, H, W);
+  B200_LAUNCH_CHECK("maxpool2_nc8_kernel");
+  return B200_OK;
+}
 
 extern "C" long long b200_upsample_add_nc8_workspace_bytes(int N, int C, int D, int H, int W, int scale) {
   if (N <= 0 || C <= 0 || C % 8 || D <= 0 || H <= 0 || W <= 0 || (scale != 1 && scale != 2)) return -1;

@@ -1,4 +1,4 @@
-"""`TcNet`: the mixin every network with a tensor-core forward (UNet, SwinUNETR, UNETR, DynUNet, SegResNet) inherits.
+"""`TcNet`: the mixin every network with a tensor-core forward (UNet, BasicUNet, SwinUNETR, UNETR, DynUNet, SegResNet) inherits.
 
 It owns what those networks share:
   * `forward`: the choice between `_forward_tc` (fp16 channel-blocked "NC8" buffers on Hopper tensor cores) and `_forward_generic`
@@ -14,7 +14,10 @@ It owns what those networks share:
     conv3x3x3_tc, a stride-1 kernel of 3x3 in one plane and 1 along the third axis on conv3x3_tc, a kernel with stride 2 on any axis
     on conv_gather_tc (per axis), and a stride-1 1x1x1 kernel on gemm_tc.  eps, gamma / beta and the slope are read from the block; the
     non-affine blocks of the transformer segmenters (eps 1e-5, slope 0.01) pass no gamma / beta, so their kernels run the
-    non-affine instantiations.
+    non-affine instantiations;
+  * for the `Convolution` blocks of UNet and BasicUNet: the reader of a block's ADN (eps, gamma / beta, activation and slope) and
+    the norm_act_nc8 pass that applies it; for SegResNet and BasicUNet: the output head after a norm + activation, fused into
+    head_conv_norm_nc8 up to 16 outputs and on gemm_tc with zero-padded columns above.
 
 A network calls `self._tc_setup()` in its constructor and supplies `_forward_tc` and `_forward_generic`."""
 from __future__ import annotations
@@ -152,6 +155,19 @@ class TcNet:
         params = [weight] + ([bias] if bias is not None else [])
         return self._cache.get(("qkvs", key, weight.device), params, build)
 
+    def _whead(self, conv: nn.Conv3d, npad: int):
+        """The 1x1x1 output convolution with its output channels zero-padded to `npad`: (packed weight, float32 bias)."""
+        def build():
+            w = torch.zeros((npad, conv.in_channels), device=conv.weight.device, dtype=torch.float32)
+            w[: conv.out_channels] = conv.weight.detach().float().reshape(conv.out_channels, -1)
+            b = torch.zeros(npad, device=conv.weight.device, dtype=torch.float32)
+            if conv.bias is not None:
+                b[: conv.out_channels] = conv.bias.detach().float()
+            return K.gemm_tc_pack_weight(w), b
+
+        params = [conv.weight] + ([conv.bias] if conv.bias is not None else [])
+        return self._cache.get(("head", npad, conv.weight.device), params, build)
+
     def _w33(self, conv: nn.Conv3d, key: str, axis: int, cin_pad: int | None = None):
         return self._cache.get(("w33", key, axis, cin_pad, conv.weight.device), [conv.weight],
                                lambda: K.conv3x3_tc_pack_weight(self._pad_cin(conv.weight, cin_pad), axis))
@@ -176,6 +192,37 @@ class TcNet:
         if norm.affine:
             return float(norm.eps), norm.weight, norm.bias
         return float(norm.eps), None, None
+
+    @staticmethod
+    def _bn(blk: nn.Module):
+        n = getattr(getattr(blk, "adn", None), "N", None)
+        return n if isinstance(n, nn.BatchNorm3d) else None
+
+    def _act_of(self, conv: nn.Module):
+        """(act code, slope) of the activation of a `Convolution` block's ADN; a PReLU's single weight is read once per value."""
+        act = getattr(conv.adn, "A", None)
+        if isinstance(act, nn.PReLU):
+            return L.ACT_LEAKY, self._cache.get(("slope", id(act)), [act.weight], lambda: float(act.weight.detach().float().item()))
+        if isinstance(act, nn.LeakyReLU):
+            return L.ACT_LEAKY, float(act.negative_slope)
+        if isinstance(act, nn.ReLU):
+            return L.ACT_RELU, 0.0
+        return L.ACT_NONE, 0.0
+
+    def _adn(self, blk: nn.Module):
+        """(instance norm?, eps, gamma, beta, act, slope) of an "NDA" `Convolution` block; a BatchNorm block has no norm left to
+        apply (it is folded into the convolution)."""
+        act, slope = self._act_of(blk)
+        if self._bn(blk) is not None:
+            return False, 1e-5, None, None, act, slope
+        eps, g, b = self._norm(blk.adn.N)
+        return True, eps, g, b, act, slope
+
+    def _finish(self, y: K.NC8, C_: int, st, blk: nn.Module, out=None, out_coff: int = 0, res=None, res_coff: int = 0) -> K.NC8:
+        """act(norm(y)) of the "NDA" block `blk` (+ res after the activation) into `out`."""
+        inorm, eps, g, b, act, slope = self._adn(blk)
+        return K.norm_act_nc8(y, C_, st if inorm else None, res=res, res_coff=res_coff, act=act, slope=slope, out=out, out_coff=out_coff,
+                              eps=eps, gamma=g, beta=b, res_after_act=res is not None)
 
     @staticmethod
     def _slope(blk: nn.Module) -> float:
@@ -306,6 +353,20 @@ class TcNet:
         skip, then the residual block runs on `cat`."""
         self._up(x, cin, block.transp_conv.conv, key, out=cat)
         return self._res_block(cat, cat.C, 0, block.conv_block, key + ".rb", defer_tail=defer_tail)
+
+    def _norm_act_head(self, x: K.NC8, stats: torch.Tensor, eps: float, gamma, beta, act: int, slope: float, conv: nn.Conv3d,
+                       dtype: torch.dtype) -> torch.Tensor:
+        """conv(act(norm(x))) for the whole NC8 image x and a 1x1x1 `conv`, as NCDHW logits in `dtype`.  Up to 16 outputs: one
+        head_conv_norm_nc8 launch with the norm and the activation (ReLU as slope 0) on its operand load.  More: norm_act_nc8,
+        then gemm_tc with the output channels zero-padded to a multiple of 16."""
+        if conv.out_channels <= 16:
+            return K.head_conv_norm_nc8(x, stats, None, 0, None, slope, eps, conv.weight, conv.bias, out_dtype=dtype, gamma=gamma, beta=beta)
+        npad = (conv.out_channels + 15) // 16 * 16
+        xn = K.norm_act_nc8(x, x.C, stats, act=act, slope=slope, eps=eps, gamma=gamma, beta=beta)
+        wp, bp = self._whead(conv, npad)
+        y, _ = K.gemm_tc(xn, wp, x.C, npad, bias=bp)
+        # the padding channels are dropped by a view (the graph replay returns a contiguous copy)
+        return K.unpack_nc8(y, dtype=dtype).narrow(1, 0, conv.out_channels)
 
     def _tail_head(self, tail, block: nn.Module, out_conv: nn.Conv3d, dtype: torch.dtype) -> torch.Tensor:
         """The 1x1x1 output convolution with the deferred tail of the last block (`defer_tail=True`) -- its norm2, the residual

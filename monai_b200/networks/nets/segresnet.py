@@ -160,19 +160,6 @@ class SegResNet(TcNet, nn.Module):
         return K.conv3x3x3_tc(y1, self._w3(blk.conv2.conv, key + ".c2"), C, C, bias=blk.conv2.conv.bias, want_stats=True,
                               in_norm=(s2, e2, *act), in_affine=(g2, b2), add=(x, 0))
 
-    def _whead(self, conv: nn.Conv3d, npad: int):
-        """The 1x1x1 output convolution with its output channels zero-padded to `npad`: (packed weight, float32 bias)."""
-        def build():
-            w = torch.zeros((npad, conv.in_channels), device=conv.weight.device, dtype=torch.float32)
-            w[: conv.out_channels] = conv.weight.detach().float().reshape(conv.out_channels, -1)
-            b = torch.zeros(npad, device=conv.weight.device, dtype=torch.float32)
-            if conv.bias is not None:
-                b[: conv.out_channels] = conv.bias.detach().float()
-            return K.gemm_tc_pack_weight(w), b
-
-        params = [conv.weight] + ([conv.bias] if conv.bias is not None else [])
-        return self._cache.get(("head", npad, conv.weight.device), params, build)
-
     def _forward_tc(self, x_in: torch.Tensor) -> torch.Tensor:
         """SegResNet.forward (segresnet.py encode + decode, eval mode) on fp16 NC8 buffers and tensor cores; the output is fp16.
 
@@ -218,12 +205,4 @@ class SegResNet(TcNet, nn.Module):
                 return K.unpack_nc8(x, dtype=x_in.dtype)
             norm, act, conv = self.conv_final[0], self.conv_final[1], self.conv_final[2].conv
             sf, eps, g, b = self._norm_tc(norm, st, n, f0)
-            a, slope = self._act_tc(act)
-            if conv.out_channels <= 16:   # norm + act applied on the head's operand load
-                return K.head_conv_norm_nc8(x, sf, None, 0, None, slope, eps, conv.weight, conv.bias, out_dtype=x_in.dtype, gamma=g, beta=b)
-            npad = (conv.out_channels + 15) // 16 * 16
-            xn = K.norm_act_nc8(x, f0, sf, act=a, slope=slope, eps=eps, gamma=g, beta=b)
-            wp, bp = self._whead(conv, npad)
-            y, _ = K.gemm_tc(xn, wp, f0, npad, bias=bp)
-            # the padding channels are dropped by a view (the graph replay returns a contiguous copy)
-            return K.unpack_nc8(y, dtype=x_in.dtype).narrow(1, 0, conv.out_channels)
+            return self._norm_act_head(x, sf, eps, g, b, *self._act_tc(act), conv, x_in.dtype)

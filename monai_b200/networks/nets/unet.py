@@ -181,16 +181,6 @@ class UNet(TcNet, nn.Module):
             raise ValueError(f"UNet with strides {tuple(self.strides[: len(self.channels) - 1])} needs spatial sizes divisible by {div}, "
                              f"got {tuple(x.shape[2:])}")
 
-    def _act_of(self, conv: Convolution):
-        act = getattr(conv.adn, "A", None)
-        if isinstance(act, nn.PReLU):
-            return L.ACT_LEAKY, self._cache.get(("slope", id(act)), [act.weight], lambda: float(act.weight.detach().float().item()))
-        if isinstance(act, nn.LeakyReLU):
-            return L.ACT_LEAKY, float(act.negative_slope)
-        if isinstance(act, nn.ReLU):
-            return L.ACT_RELU, 0.0
-        return L.ACT_NONE, 0.0
-
     def _tc_conv(self, conv: Convolution, x, cin: int, in_coff: int, out, out_coff: int, raw=None):
         """Convolution block (conv + InstanceNorm + activation) on tensor cores; result goes to out[:, out_coff:...]."""
         m = conv.conv
@@ -242,11 +232,6 @@ class UNet(TcNet, nn.Module):
     # is a fixed per-channel affine: it is folded into the convolution's weight and bias, and its unit's activation runs on
     # norm_act_nc8 without statistics.  An InstanceNorm takes its statistics from the convolution epilogues and is applied on the
     # next convolution's operand load where that kernel allows the slope (in [0, 1]), else materialised by norm_act_nc8.
-    @staticmethod
-    def _bn(blk: nn.Module):
-        n = getattr(getattr(blk, "adn", None), "N", None)
-        return n if isinstance(n, nn.BatchNorm3d) else None
-
     @staticmethod
     def _tensors(*mods) -> list:
         """The tensors a packed weight depends on: weight and bias of convolutions and norms, and a BatchNorm's running statistics
@@ -337,24 +322,10 @@ class UNet(TcNet, nn.Module):
             return t
         return self._cache.get(("pad", id(t), n), [t], lambda: torch.nn.functional.pad(t.detach().float(), (0, n - t.numel())))
 
-    def _adn(self, blk: Convolution):
-        """(instance norm?, eps, gamma, beta, act, slope) of an "NDA" block; a BatchNorm block has no norm left to apply."""
-        act, slope = self._act_of(blk)
-        if self._bn(blk) is not None:
-            return False, 1e-5, None, None, act, slope
-        eps, g, b = self._norm(blk.adn.N)
-        return True, eps, g, b, act, slope
-
     @staticmethod
     def _on_load(inorm: bool, act: int, slope: float) -> bool:
         """Whether conv3x3x3_tc can apply this norm + activation on its operand load (it takes slopes in [0, 1] only)."""
         return inorm and (act != L.ACT_LEAKY or 0.0 <= slope <= 1.0)
-
-    def _finish(self, y: K.NC8, C_: int, st, blk: Convolution, out=None, out_coff: int = 0, res=None, res_coff: int = 0) -> K.NC8:
-        """act(norm(y)) of `blk` (+ res after the activation) into `out`."""
-        inorm, eps, g, b, act, slope = self._adn(blk)
-        return K.norm_act_nc8(y, C_, st if inorm else None, res=res, res_coff=res_coff, act=act, slope=slope, out=out, out_coff=out_coff,
-                              eps=eps, gamma=g, beta=b, res_after_act=res is not None)
 
     def _tc_ru(self, ru: ResidualUnit, x, cin: int, in_coff: int, out: K.NC8, out_coff: int, raw=None, cin_pad: int | None = None) -> None:
         """A ResidualUnit with an "NDA" last unit: out[:, out_coff:...] = act(norm(y_last)) + residual(x)."""

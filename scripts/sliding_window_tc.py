@@ -14,9 +14,11 @@
   * segresnet wholebody: init_filters 32, 1 input channel, 105 outputs, GroupNorm(8); a 256^3 fp16 volume, roi 96^3;
   * unet res_batch:      the spleen CT UNet of MONAI's tutorial and bundle (channels 16 ... 256, strides 2, two residual units,
                          eval-mode BatchNorm, PReLU, 1 -> 2 channels); a 256^3 fp16 volume, roi 160^3;
-  * unet res_instance:   the same net with InstanceNorm (MONAI's default norm); a 256^3 fp16 volume, roi 96^3.
+  * unet res_instance:   the same net with InstanceNorm (MONAI's default norm); a 256^3 fp16 volume, roi 96^3;
+  * basic_unet:          the reference's defaults (features 32, 32, 64, 128, 256, 32, affine instance norm, LeakyReLU 0.1, 1 -> 2
+                         channels); a 256^3 fp16 volume, roi 96^3.
 
-    python scripts/sliding_window_tc.py --net unetr|dynunet|segresnet|unet [--workload brats|wholebody|both (SegResNet) |
+    python scripts/sliding_window_tc.py --net unetr|dynunet|segresnet|unet|basic_unet [--workload brats|wholebody|both (SegResNet) |
                                         iso|aniso_d|aniso_w|all (DynUNet) | res_batch|res_instance|res (UNet)] [--sw-batch 4]
                                         [--steps 3] [--warmup 1]
 
@@ -24,8 +26,8 @@ Overlap 0.5, gaussian blending.  Every batch shape (the full batches and the rem
 is bracketed by CUDA events with a 256 MiB L2 flush before it (outside the timed interval), and the spread of the timed steps is
 reported.  A separate profiled step lists device time per kernel.  Finally one forward of sw_batch windows and one of a single
 window are timed on each path: `net(x)` (tensor cores) and `net._forward_generic(x)` (the generic CUDA-core kernels), giving the
-speed-up per window without running a whole volume on CUDA cores; for UNet the tensor-core forward is also timed per window eager
-(without CUDA-graph replay), and with BatchNorm the activation-only norm_act_nc8 passes of one forward are timed on their own.
+speed-up per window without running a whole volume on CUDA cores; for UNet and BasicUNet the tensor-core forward is also timed per
+window in its other launch mode (eager or CUDA-graph replay), and with BatchNorm the activation-only norm_act_nc8 passes of one forward are timed on their own.
 Prints one JSON line per workload, with the card name and power limit read in the same run.
 """
 from __future__ import annotations
@@ -165,6 +167,22 @@ def unet_flops(net, roi) -> dict:
     return {"encoder": enc, "decoder": dec, "total": enc + dec}
 
 
+def basic_unet_flops(net, roi) -> dict:
+    """Multiply-add FLOPs (x2) of one window, from the layer shapes of BasicUNet.forward: the two 3x3x3 convolutions of every TwoConv
+    (encoder: conv_0 and down_1 ... down_4; decoder: upcat_4 ... upcat_1), the transposed convolutions k2 s2 and the 1x1x1 head."""
+    v = [math.prod(s // 2**k for s in roi) for k in range(5)]   # voxels at level k
+
+    def two(tc, n):
+        return sum(2.0 * n * 27 * c.conv.in_channels * c.conv.out_channels for c in (tc.conv_0, tc.conv_1))
+
+    enc = two(net.conv_0, v[0]) + sum(two(d.convs, v[k]) for k, d in enumerate((net.down_1, net.down_2, net.down_3, net.down_4), 1))
+    dec = 2.0 * v[0] * net.final_conv.in_channels * net.final_conv.out_channels
+    for k, uc in zip((3, 2, 1, 0), (net.upcat_4, net.upcat_3, net.upcat_2, net.upcat_1)):   # uc lands on level k
+        dc = uc.upsample.deconv
+        dec += 2.0 * v[k + 1] * 8 * dc.in_channels * dc.out_channels + two(uc.convs, v[k])
+    return {"encoder": enc, "decoder": dec, "total": enc + dec}
+
+
 def unet_act_passes(net, roi, batch) -> list:
     """(channels, spatial size) of each activation-only norm_act_nc8 pass of a BatchNorm residual UNet forward: the output of every
     unit of a down or bottom ResidualUnit but its last, activated before the next unit's convolution reads it."""
@@ -181,7 +199,7 @@ def unet_act_passes(net, roi, batch) -> list:
 
 
 def _nets():
-    from monai_b200.networks.nets import UNETR, DynUNet, SegResNet, UNet
+    from monai_b200.networks.nets import UNETR, BasicUNet, DynUNet, SegResNet, UNet
 
     return {
         "unetr": {
@@ -220,6 +238,11 @@ def _nets():
                 make=lambda: UNet(3, 1, 2, (16, 32, 64, 128, 256), (2, 2, 2, 2), num_res_units=2), seed=20, cin=1,
                 volume=(256, 256, 256), roi=(96, 96, 96), flops=unet_flops, eager_vs_replay=True,
                 desc="UNet(in=1, out=2, channels 16..256, strides 2, num_res_units=2, InstanceNorm, PReLU)"),
+        },
+        "basic_unet": {
+            "basic_unet_sliding_window": dict(
+                make=lambda: BasicUNet(), seed=70, cin=1, volume=(256, 256, 256), roi=(96, 96, 96), flops=basic_unet_flops, eager_vs_replay=True,
+                desc="BasicUNet(in=1, out=2, features (32, 32, 64, 128, 256, 32), affine IN, LeakyReLU 0.1)"),
         },
     }
 
@@ -350,7 +373,7 @@ def run(metric: str, wl: dict, args, card: dict) -> dict:
 
 def main() -> None:
     ap = argparse.ArgumentParser()
-    ap.add_argument("--net", required=True, choices=["unetr", "dynunet", "segresnet", "unet"])
+    ap.add_argument("--net", required=True, choices=["unetr", "dynunet", "segresnet", "unet", "basic_unet"])
     ap.add_argument("--workload", default=None, choices=["both", "brats", "wholebody", "all", "iso", "aniso_d", "aniso_w", "res_batch",
                                                           "res_instance", "res"],
                     help="SegResNet: brats|wholebody|both (default both); DynUNet: iso|aniso_d|aniso_w|all (default iso); "
