@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 6
+#define B200_ABI_VERSION 7
 
 /* ---- library ---------------------------------------------------------------------------------------- */
 int b200_abi_version(void);
@@ -191,6 +191,13 @@ typedef struct b200_conv_tc_desc {
   float in_eps;
   int in_act;               /* 0 none, 1 leaky-relu (in_slope), 3 relu */
   float in_slope;
+  /* GIVEN operand normalisation (ABI 7; 0 = off; in the 4 bytes that were padding, so the descriptor keeps its 128-byte layout):
+   * in_table = 1 makes in_stats a float32 device [Cin][2] table of {scale, shift}, 8-byte aligned and the same for every batch item,
+   * and the kernel feeds act(x * scale + shift) with in_act / in_slope as above.  An eval-mode BatchNorm in front of the
+   * convolution (scale = gamma / sqrt(running_var + eps), shift = beta - running_mean * scale; SegResNetDS's SegResBlock,
+   * segresnet_ds.py:121-125), which cannot be folded into the weights when x is also the identity branch.  Needs in_stats, excludes
+   * in_gamma / in_beta; like the statistics form it serves the epilogue add. */
+  int in_table;
   /* Folded 1x1x1 residual convolution (round 2; res_w == NULL = off; exclusive with in_stats; Cout <= 128): UnetResBlock.conv3
    * (dynunet_block.py:75-87, 104-108) reads the same input as conv1, so res_y = conv1x1x1(x, W3) is produced by the same launch
    * (one extra MMA per output plane and K slice on the centre view of the staged halo tile).  res_w = b200_gemm_tc_pack_weight image
@@ -233,9 +240,9 @@ int b200_conv3x3x3_tc(const b200_conv_tc_desc* desc, const void* x, const void* 
  * size 1 -- kernels [1,3,3], [3,1,3] and [3,3,1], zero padding (k - 1) / 2 per axis -- the high-resolution convolutions of
  * anisotropic nnU-Net / DynUNet plans.  The same kernel as b200_conv3x3x3_tc without the dead taps; its result equals
  * b200_conv3x3x3_tc with the weight zero-padded to 3x3x3, bit for bit.  Takes the b200_conv_tc_desc of b200_conv3x3x3_tc with the
- * plain and the operand-normalising forms (in_stats, optionally in_gamma / in_beta); res_w and add return B200_ERR_UNSUPPORTED and
- * the workspace query returns -1 for them.  The weight is the Conv3d weight [Cout,Cin,kd,kh,kw] float32 (device) with the axis of
- * size 1 (9 * Cin * Cout values). */
+ * plain and the operand-normalising forms (in_stats, optionally in_gamma / in_beta or in_table) and, since ABI 7, the
+ * epilogue add; res_w returns B200_ERR_UNSUPPORTED and the workspace query returns -1 for it.  The weight is the Conv3d weight
+ * [Cout,Cin,kd,kh,kw] float32 (device) with the axis of size 1 (9 * Cin * Cout values). */
 long long b200_conv3x3_tc_weight_bytes(int Cin, int Cout);
 int b200_conv3x3_tc_pack_weight(const float* w, int Cin, int Cout, int axis, void* packed, void* stream);
 long long b200_conv3x3_tc_workspace_bytes(const b200_conv_tc_desc* desc, int axis);

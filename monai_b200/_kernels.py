@@ -552,6 +552,7 @@ def conv3x3x3_tc(
     out: NC8 | None = None, out_coff: int = 0, want_stats: bool = False,
     in_norm: tuple[torch.Tensor, float, int, float] | None = None, res_w: torch.Tensor | None = None,
     in_affine: tuple[torch.Tensor | None, torch.Tensor | None] | None = None, add: tuple[NC8, int] | None = None,
+    in_scale_shift: tuple[torch.Tensor, int, float] | None = None,
 ):
     """3x3x3 / stride 1 / pad 1 convolution.  `in_norm` = (stats, eps, act, slope): x is the RAW output of the previous
     convolution and InstanceNorm + activation are applied on the operand load (no norm_act pass in between).
@@ -559,7 +560,9 @@ def conv3x3x3_tc(
     `res_w` = gemm_tc_pack_weight image of a 1x1x1 convolution [Cout, Cin] of the SAME input: it is computed by the same launch
     and the call returns (out, stats, res_out, res_stats) instead of (out, stats).
     `add` = (NC8 tensor, channel offset): channels [coff, coff + Cout) of it, with the output's shape, are added to the result in
-    fp32 before its fp16 store, and the statistics are those of the sum; it needs `in_norm`."""
+    fp32 before its fp16 store, and the statistics are those of the sum; it needs `in_norm` or `in_scale_shift`.
+    `in_scale_shift` = (table, act, slope): the operand load feeds act(x * scale + shift) with the given float32 [Cin, 2] {scale, shift}
+    table (an eval-mode BatchNorm, `batchnorm_scale_shift`) instead of a table derived from statistics; it excludes `in_norm`."""
     if out is None:
         out = NC8(x.N, Cout, x.sp, x.buf.device)
     dev = x.buf.device
@@ -584,14 +587,13 @@ def conv3x3x3_tc(
         raise ValueError("conv3x3x3_tc: in_affine needs in_norm")
     d.in_gamma, d.in_beta = L.ptr(g32), L.ptr(be32)
     label = "conv3x3x3_tc_affine" if g32 is not None or be32 is not None else "conv3x3x3_tc"
+    _set_scale_shift(d, "conv3x3x3_tc", in_scale_shift, in_norm, Cin, dev)
+    if res_w is not None and in_scale_shift is not None:
+        raise ValueError("conv3x3x3_tc: res_w excludes in_scale_shift")
     if add is not None:
-        a, a_coff = add
-        if in_norm is None or res_w is not None:
-            raise ValueError("conv3x3x3_tc: add needs in_norm and excludes res_w")
-        if a.N != x.N or a.sp != x.sp or a_coff % 8 or a_coff + Cout > a.C:
-            raise ValueError(f"conv3x3x3_tc: add must be a channel slice of an NC8 tensor of the output's shape, got {a.C} channels at "
-                             f"{a.sp} (offset {a_coff}) for {Cout} channels at {x.sp}")
-        d.add, d.add_ctot, d.add_coff = L.ptr(a.buf), a.C, int(a_coff)
+        if res_w is not None:
+            raise ValueError("conv3x3x3_tc: add excludes res_w")
+        _set_add(d, "conv3x3x3_tc", add, in_norm, in_scale_shift, x, Cout)
         label = "conv3x3x3_tc_affine_add"
     ws = _ws(L.load().b200_conv3x3x3_tc_workspace_bytes(C.byref(d)), dev) if want_stats else None
     _call("conv3x3x3_tc", C.byref(d), L.ptr(x.buf), L.ptr(packed_w), L.ptr(b32), L.ptr(out.buf), L.ptr(stats), L.ptr(ws), L.stream_ptr(dev),
@@ -622,10 +624,12 @@ def conv3x3_tc(
     x: NC8, packed_w: torch.Tensor, Cin: int, Cout: int, axis: int, in_coff: int = 0, bias: torch.Tensor | None = None,
     out: NC8 | None = None, out_coff: int = 0, want_stats: bool = False,
     in_norm: tuple[torch.Tensor, float, int, float] | None = None,
-    in_affine: tuple[torch.Tensor | None, torch.Tensor | None] | None = None,
+    in_affine: tuple[torch.Tensor | None, torch.Tensor | None] | None = None, add: tuple[NC8, int] | None = None,
+    in_scale_shift: tuple[torch.Tensor, int, float] | None = None,
 ):
     """Stride-1 convolution whose kernel is 1 along `axis` and 3 along the other two (padding 0 / 1 / 1 accordingly), e.g. the
-    [1, 3, 3] convolutions of anisotropic DynUNet plans.  `in_norm` / `in_affine` as in conv3x3x3_tc.  Returns (out, stats)."""
+    [1, 3, 3] convolutions of anisotropic DynUNet plans.  `in_norm`, `in_affine`, `in_scale_shift` and `add` as in conv3x3x3_tc.
+    Returns (out, stats)."""
     if out is None:
         out = NC8(x.N, Cout, x.sp, x.buf.device)
     dev = x.buf.device
@@ -642,11 +646,50 @@ def conv3x3_tc(
     if (g32 is not None or be32 is not None) and in_norm is None:
         raise ValueError("conv3x3_tc: in_affine needs in_norm")
     d.in_gamma, d.in_beta = L.ptr(g32), L.ptr(be32)
+    label = "conv3x3_tc_affine" if g32 is not None or be32 is not None else "conv3x3_tc"
+    _set_scale_shift(d, "conv3x3_tc", in_scale_shift, in_norm, Cin, dev)
+    if add is not None:
+        _set_add(d, "conv3x3_tc", add, in_norm, in_scale_shift, x, Cout)
+        label = "conv3x3_tc_affine_add"
     ws = _ws(L.load().b200_conv3x3_tc_workspace_bytes(C.byref(d), int(axis)), dev) if want_stats else None
     _call("conv3x3_tc", C.byref(d), int(axis), L.ptr(x.buf), L.ptr(packed_w), L.ptr(b32), L.ptr(out.buf), L.ptr(stats), L.ptr(ws),
-          L.stream_ptr(dev), flops=2.0 * x.N * x.S * Cin * Cout * 9, nbytes=float(x.N * x.S * (Cin + Cout) * 2) + _nb(packed_w),
-          label="conv3x3_tc_affine" if g32 is not None or be32 is not None else "conv3x3_tc")
+          L.stream_ptr(dev), flops=2.0 * x.N * x.S * Cin * Cout * 9,
+          nbytes=float(x.N * x.S * (Cin + Cout * (2 if add is not None else 1)) * 2) + _nb(packed_w), label=label)
     return out, stats
+
+
+def _set_scale_shift(d, name: str, in_scale_shift, in_norm, Cin: int, dev) -> None:
+    """Fill the in_stats (the table) / in_table / in_act / in_slope fields of a b200_conv_tc_desc from (table, act, slope)."""
+    if in_scale_shift is None:
+        return
+    tab, act, slope = in_scale_shift
+    if in_norm is not None:
+        raise ValueError(f"{name}: in_scale_shift excludes in_norm and in_affine")
+    if tab.dtype != torch.float32 or tab.numel() != Cin * 2 or not tab.is_contiguous() or tab.device != dev:
+        raise ValueError(f"{name}: in_scale_shift must be a contiguous float32 [Cin, 2] tensor on the input's device")
+    d.in_stats, d.in_table, d.in_act, d.in_slope = L.ptr(tab), 1, int(act), float(slope)
+
+
+def _set_add(d, name: str, add: tuple[NC8, int], in_norm, in_scale_shift, x: NC8, Cout: int) -> None:
+    """Fill the add fields of a b200_conv_tc_desc: channels [coff, coff + Cout) of an NC8 tensor of the output's shape."""
+    a, a_coff = add
+    if in_norm is None and in_scale_shift is None:
+        raise ValueError(f"{name}: add needs in_norm or in_scale_shift")
+    if a.N != x.N or a.sp != x.sp or a_coff % 8 or a_coff + Cout > a.C:
+        raise ValueError(f"{name}: add must be a channel slice of an NC8 tensor of the output's shape, got {a.C} channels at "
+                         f"{a.sp} (offset {a_coff}) for {Cout} channels at {x.sp}")
+    d.add, d.add_ctot, d.add_coff = L.ptr(a.buf), a.C, int(a_coff)
+
+
+def batchnorm_scale_shift(bn: torch.nn.Module) -> torch.Tensor:
+    """The float32 [C, 2] {scale, shift} table of an eval-mode BatchNorm: s = gamma / sqrt(running_var + eps), t = beta - mean * s."""
+    s = 1.0 / torch.sqrt(bn.running_var.detach().float() + float(bn.eps))
+    if bn.affine:
+        s = bn.weight.detach().float() / torch.sqrt(bn.running_var.detach().float() + float(bn.eps))
+    t = -bn.running_mean.detach().float() * s
+    if bn.affine:
+        t = t + bn.bias.detach().float()
+    return torch.stack((s, t), dim=1).contiguous()
 
 
 def norm_act_cin1res_nc8(x: NC8, C_: int, stats: torch.Tensor, raw: torch.Tensor, raw_stats: torch.Tensor, raw_weight: torch.Tensor,

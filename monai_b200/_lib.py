@@ -14,7 +14,7 @@ import torch
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = _HERE / "lib" / "libmonai_b200.so"
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 DT_F32, DT_F16 = 0, 1
 _DT = {torch.float32: DT_F32, torch.float16: DT_F16}
 
@@ -50,7 +50,7 @@ class ConvTcDesc(C.Structure):
     _fields_ = [
         ("N", i32), ("Cin", i32), ("Cout", i32), ("D", i32), ("H", i32), ("W", i32),
         ("in_ctot", i32), ("in_coff", i32), ("out_ctot", i32), ("out_coff", i32),
-        ("in_stats", vp), ("in_eps", f32), ("in_act", i32), ("in_slope", f32),
+        ("in_stats", vp), ("in_eps", f32), ("in_act", i32), ("in_slope", f32), ("in_table", i32),
         ("res_w", vp), ("res_y", vp), ("res_ctot", i32), ("res_coff", i32), ("res_stats", vp),
         ("in_gamma", vp), ("in_beta", vp), ("add", vp), ("add_ctot", i32), ("add_coff", i32),
     ]

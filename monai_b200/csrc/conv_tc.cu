@@ -185,19 +185,22 @@ struct ConvTcAdd { const __half* x; int ctot, coff; };
 //
 // ADD (with NORM only): y = conv(act(norm(x))) + add, the sum formed in fp32 in the epilogue before the fp16 store, and the statistics
 // are those of the sum -- conv2 plus the identity of a pre-activation residual block (SegResNet's ResBlock,
-// monai/networks/blocks/segresnet_block.py:83-94).  The body is shared by conv3x3x3_tc_kernel (ADD = false: the code it always
-// had) and conv3x3x3_tc_add_kernel.
+// monai/networks/blocks/segresnet_block.py:83-94; SegResNetDS's SegResBlock, segresnet_ds.py:121-125).  The body is shared by
+// conv3x3x3_tc_kernel (ADD = false: the code it always had), conv3x3x3_tc_add_kernel and conv3x3_tc_add_kernel.
+//
+// NORM: 0 = off, 1 = the (scale, shift) table derived from in_stats, 2 = the table given in in_stats (d.in_table = 1: an eval-mode BatchNorm,
+// the same for every batch item); the transform is the same.
 //
 // KF (kernel form): kForm333, or a one-plane 3x3 kernel of b200_conv3x3_tc (see kFormD1 / kFormHW1; `axis` = 1 or 2 names the
 // axis of size 1 of kFormHW1).  The live MMAs of each accumulator run in the order of the 3x3x3 form, so a one-plane kernel gives the
 // bits of the 3x3x3 form with zero-padded weights.
-template <int NT, int BD, bool NORM, bool RES, bool ADD, int KF = kForm333>
+template <int NT, int BD, int NORM, bool RES, bool ADD, int KF = kForm333>
 __device__ __forceinline__ void conv3x3x3_tc_body(const CUtensorMap& tmap, const ConvTcParams& p, const ConvTcAffine& aff,
                                                   const ConvTcAdd& add, int axis = 0) {
   using Cfg = ConvTcCfg<NT, BD, RES, KF>;
   static_assert(!(NORM && RES), "the residual fold is used by conv1, the operand normalisation by conv2");
   static_assert(!ADD || (NORM && !RES), "the epilogue add is a variant of the operand-normalising instantiations");
-  static_assert(KF == kForm333 || !(RES || ADD), "the one-plane kernels have the plain and the operand-normalising forms only");
+  static_assert(KF == kForm333 || !RES, "the one-plane kernels have no folded residual");
   constexpr int kSA = Cfg::kSA, kSB = Cfg::kSB;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = tc::align_smem128(smem_raw);   // keeps the shared address space (LDS/STS, not generic LD/ST)
@@ -381,9 +384,14 @@ __device__ __forceinline__ void conv3x3x3_tc_body(const CUtensorMap& tmap, const
       const ConvTile c = conv_tile<BD>(p.e, t);
       if (c.n != table_n) {
         tc::named_bar(1, 96);          // every transform thread is done with the previous item's table
-        const float* st = p.in_stats + 2 * (long long)c.n * d.Cin;
-        for (int ch = tt; ch < d.Cin; ch += 96)   // the helper of norm_act_nc8_kernel: same (scale, shift) bits
-          reinterpret_cast<float2*>(s_norm)[ch] = instnorm_scale_shift(__ldg(st + 2 * ch), __ldg(st + 2 * ch + 1), invS, eps, aff.gamma, aff.beta, ch);
+        if constexpr (NORM == 2) {     // the given table, the same for every item
+          for (int ch = tt; ch < d.Cin; ch += 96)
+            reinterpret_cast<float2*>(s_norm)[ch] = __ldg(reinterpret_cast<const float2*>(p.in_stats) + ch);
+        } else {
+          const float* st = p.in_stats + 2 * (long long)c.n * d.Cin;
+          for (int ch = tt; ch < d.Cin; ch += 96)   // the helper of norm_act_nc8_kernel: same (scale, shift) bits
+            reinterpret_cast<float2*>(s_norm)[ch] = instnorm_scale_shift(__ldg(st + 2 * ch), __ldg(st + 2 * ch + 1), invS, eps, aff.gamma, aff.beta, ch);
+        }
         tc::named_bar(1, 96);
         table_n = c.n;
       }
@@ -432,24 +440,32 @@ __device__ __forceinline__ void conv3x3x3_tc_body(const CUtensorMap& tmap, const
   }
 }
 
-template <int NT, int BD, bool NORM, bool RES>
+template <int NT, int BD, int NORM, bool RES>
 __global__ void __launch_bounds__(ConvTcCfg<NT, BD, RES>::kThreads, 1) conv3x3x3_tc_kernel(const __grid_constant__ CUtensorMap tmap, ConvTcParams p,
                                                                                                   ConvTcAffine aff) {
   conv3x3x3_tc_body<NT, BD, NORM, RES, false>(tmap, p, aff, ConvTcAdd{nullptr, 0, 0});
 }
 
 // the one-plane 3x3 convolution (b200_conv3x3_tc): KF = kFormD1 or kFormHW1, plain or operand-normalising
-template <int NT, int BD, bool NORM, int KF>
+template <int NT, int BD, int NORM, int KF>
 __global__ void __launch_bounds__(ConvTcCfg<NT, BD, false, KF>::kThreads, 1) conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmap, ConvTcParams p,
                                                                                                    ConvTcAffine aff, int axis) {
   conv3x3x3_tc_body<NT, BD, NORM, false, false, KF>(tmap, p, aff, ConvTcAdd{nullptr, 0, 0}, axis);
 }
 
-template <int NT, int BD>
+// the one-plane 3x3 convolution with the operand normalisation and the epilogue add
+template <int NT, int BD, int NORM, int KF>
+__global__ void __launch_bounds__(ConvTcCfg<NT, BD, false, KF>::kThreads, 1) conv3x3_tc_add_kernel(const __grid_constant__ CUtensorMap tmap,
+                                                                                                       ConvTcParams p, ConvTcAffine aff,
+                                                                                                       ConvTcAdd add, int axis) {
+  conv3x3x3_tc_body<NT, BD, NORM, false, true, KF>(tmap, p, aff, add, axis);
+}
+
+template <int NT, int BD, int NORM>
 __global__ void __launch_bounds__(ConvTcCfg<NT, BD, false>::kThreads, 1) conv3x3x3_tc_add_kernel(const __grid_constant__ CUtensorMap tmap,
                                                                                                         ConvTcParams p, ConvTcAffine aff,
                                                                                                         ConvTcAdd add) {
-  conv3x3x3_tc_body<NT, BD, true, false, true>(tmap, p, aff, add);
+  conv3x3x3_tc_body<NT, BD, NORM, false, true>(tmap, p, aff, add);
 }
 
 // NC8 normalise + activation (same math as norm_act_kernel, 8 channels per 16-byte vector)
@@ -582,7 +598,7 @@ struct ConvTcCall {
   int axis;
 };
 
-template <int NT, int BD, bool NORM, bool RES = false, bool ADD = false, int KF = kForm333>
+template <int NT, int BD, int NORM, bool RES = false, bool ADD = false, int KF = kForm333>
 static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
   using Cfg = ConvTcCfg<NT, BD, RES, KF>;
   ConvTcParams p;
@@ -618,13 +634,18 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
   const int smem = Cfg::kSmemBytes + (NORM ? d.Cin * 8 : 0);   // NORM: the per-channel scale / shift table
   B200_REQUIRE(smem <= 227 * 1024, "conv3x3x3_tc: Cin %d is too wide for the operand normalisation table", d.Cin);
   const ConvTcAffine aff{d.in_gamma, d.in_beta};
-  if constexpr (KF != kForm333) {
+  if constexpr (KF != kForm333 && ADD) {
+    auto kern = conv3x3_tc_add_kernel<NT, BD, NORM, KF>;
+    B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, aff, ConvTcAdd{(const __half*)d.add, d.add_ctot, d.add_coff}, c.axis);
+    B200_LAUNCH_CHECK("conv3x3_tc_add_kernel");
+  } else if constexpr (KF != kForm333) {
     auto kern = conv3x3_tc_kernel<NT, BD, NORM, KF>;
     B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, aff, c.axis);
     B200_LAUNCH_CHECK("conv3x3_tc_kernel");
   } else if constexpr (ADD) {
-    auto kern = conv3x3x3_tc_add_kernel<NT, BD>;
+    auto kern = conv3x3x3_tc_add_kernel<NT, BD, NORM>;
     B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     kern<<<grid, Cfg::kThreads, smem, c.st>>>(tmap, p, aff, ConvTcAdd{(const __half*)d.add, d.add_ctot, d.add_coff});
     B200_LAUNCH_CHECK("conv3x3x3_tc_add_kernel");
@@ -646,21 +667,32 @@ static int launch_conv_tc(const b200_conv_tc_desc& d, ConvTcCall& c) {
 // the epilogue add holds its tile in at most 192 accumulator columns (BD * NT): the deeper ADD tiles would spill
 constexpr int kAddCols = 192;
 
+// the operand-normalising forms: the table derived from in_stats (NORM 1) or the table given in in_stats (NORM 2, d.in_table)
+template <int NT, int BD, bool ADD, int KF>
+static int launch_norm(const b200_conv_tc_desc& d, ConvTcCall& c) {
+  return d.in_table ? launch_conv_tc<NT, BD, 2, false, ADD, KF>(d, c) : launch_conv_tc<NT, BD, 1, false, ADD, KF>(d, c);
+}
+
 template <int NT, int BD>
 static int launch_variant(const b200_conv_tc_desc& d, ConvTcCall& c) {
-  if (c.axis >= 0) {   // b200_conv3x3_tc: plain or operand-normalising (its entry point rejects res_w and add)
-    if (c.axis == 0) return d.in_stats ? launch_conv_tc<NT, BD, true, false, false, kFormD1>(d, c) : launch_conv_tc<NT, BD, false, false, false, kFormD1>(d, c);
-    return d.in_stats ? launch_conv_tc<NT, BD, true, false, false, kFormHW1>(d, c) : launch_conv_tc<NT, BD, false, false, false, kFormHW1>(d, c);
+  const bool norm = d.in_stats != nullptr;
+  if (c.axis >= 0) {   // b200_conv3x3_tc: plain, operand-normalising, or with the epilogue add (its entry point rejects res_w)
+    if constexpr (BD * NT <= kAddCols) {
+      if (d.add) return c.axis == 0 ? launch_norm<NT, BD, true, kFormD1>(d, c) : launch_norm<NT, BD, true, kFormHW1>(d, c);
+    }
+    if (d.add) return set_err(B200_ERR_UNSUPPORTED, "conv3x3_tc: no epilogue-add instantiation for NT %d, BD %d", NT, BD);
+    if (norm) return c.axis == 0 ? launch_norm<NT, BD, false, kFormD1>(d, c) : launch_norm<NT, BD, false, kFormHW1>(d, c);
+    return c.axis == 0 ? launch_conv_tc<NT, BD, 0, false, false, kFormD1>(d, c) : launch_conv_tc<NT, BD, 0, false, false, kFormHW1>(d, c);
   }
   if constexpr (BD * NT <= kAddCols) {
-    if (d.add) return launch_conv_tc<NT, BD, true, false, true>(d, c);
+    if (d.add) return launch_norm<NT, BD, true, kForm333>(d, c);
   }
   if (d.add) return set_err(B200_ERR_UNSUPPORTED, "conv3x3x3_tc: no epilogue-add instantiation for NT %d, BD %d", NT, BD);
-  if (d.in_stats) return launch_conv_tc<NT, BD, true>(d, c);
+  if (norm) return launch_norm<NT, BD, false, kForm333>(d, c);
   if constexpr (NT <= 128 && 2 * BD * NT <= 256) {
-    if (d.res_w) return launch_conv_tc<NT, BD, false, true>(d, c);
+    if (d.res_w) return launch_conv_tc<NT, BD, 0, true>(d, c);
   }
-  return launch_conv_tc<NT, BD, false>(d, c);
+  return launch_conv_tc<NT, BD, 0>(d, c);
 }
 
 template <int NT>
@@ -684,17 +716,23 @@ static int conv_tc_dispatch(const b200_conv_tc_desc& d, ConvTcCall& c) {
                "conv3x3x3_tc: Cin and Cout must be multiples of 16 (got %d, %d)", d.Cin, d.Cout);
   B200_REQUIRE(d.in_ctot % 8 == 0 && d.in_coff % 8 == 0 && d.in_coff + d.Cin <= d.in_ctot, "conv3x3x3_tc: bad input channel slice");
   B200_REQUIRE(d.out_ctot % 8 == 0 && d.out_coff % 8 == 0 && d.out_coff + d.Cout <= d.out_ctot, "conv3x3x3_tc: bad output channel slice");
-  B200_REQUIRE(!d.in_stats || d.in_act == 0 || d.in_act == 1 || d.in_act == 3, "conv3x3x3_tc: in_act must be none, leaky-relu or relu");
-  B200_REQUIRE(!d.in_stats || d.in_act != 1 || (d.in_slope >= 0.f && d.in_slope <= 1.f), "conv3x3x3_tc: in_slope must lie in [0, 1] (got %g)", (double)d.in_slope);
+  const bool norm = d.in_stats != nullptr;
+  B200_REQUIRE(!norm || d.in_act == 0 || d.in_act == 1 || d.in_act == 3, "conv3x3x3_tc: in_act must be none, leaky-relu or relu");
+  B200_REQUIRE(!norm || d.in_act != 1 || (d.in_slope >= 0.f && d.in_slope <= 1.f), "conv3x3x3_tc: in_slope must lie in [0, 1] (got %g)", (double)d.in_slope);
+  B200_REQUIRE(d.in_table == 0 || d.in_table == 1, "conv3x3x3_tc: in_table must be 0 (statistics) or 1 (a given scale / shift table)");
+  if (d.in_table) {
+    B200_REQUIRE(d.in_stats && !(d.in_gamma || d.in_beta), "conv3x3x3_tc: in_table needs the table in in_stats and excludes in_gamma and in_beta");
+    B200_REQUIRE((reinterpret_cast<uintptr_t>(d.in_stats) & 7) == 0, "conv3x3x3_tc: the in_table scale / shift table must be 8-byte aligned");
+  }
   B200_REQUIRE(d.in_stats || !(d.in_gamma || d.in_beta), "conv3x3x3_tc: affine parameters of the operand normalisation without in_stats");
   if (d.add) {
-    B200_REQUIRE(d.in_stats && !d.res_w, "conv3x3x3_tc: the epilogue add needs in_stats (the operand normalisation) and no folded residual");
+    B200_REQUIRE(norm && !d.res_w, "conv3x3x3_tc: the epilogue add needs in_stats (the operand normalisation) and no folded residual");
     B200_REQUIRE(d.add_ctot % 8 == 0 && d.add_coff % 8 == 0 && d.add_coff >= 0 && d.add_coff + d.Cout <= d.add_ctot,
                  "conv3x3x3_tc: bad channel slice of the added tensor");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(d.add) & 15) == 0, "conv3x3x3_tc: the added tensor must be 16-byte aligned");
   }
   if (d.res_w) {
-    B200_REQUIRE(!d.in_stats, "conv3x3x3_tc: the folded residual convolution and the operand normalisation are exclusive");
+    B200_REQUIRE(!norm, "conv3x3x3_tc: the folded residual convolution and the operand normalisation are exclusive");
     B200_REQUIRE(d.res_y && d.Cout <= 128, "conv3x3x3_tc: the folded residual convolution needs res_y and Cout <= 128 (got %d)", d.Cout);
     B200_REQUIRE(d.res_ctot % 8 == 0 && d.res_coff % 8 == 0 && d.res_coff + d.Cout <= d.res_ctot, "conv3x3x3_tc: bad residual output channel slice");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(d.res_w) & 15) == 0 && (reinterpret_cast<uintptr_t>(d.res_y) & 15) == 0, "conv3x3x3_tc: residual pointers must be 16-byte aligned");
@@ -747,7 +785,7 @@ extern "C" int b200_conv3x3_tc_pack_weight(const float* w, int Cin, int Cout, in
 
 static int conv3x3_tc_dispatch(const b200_conv_tc_desc& d, ConvTcCall& c) {
   B200_REQUIRE(c.axis >= 0 && c.axis <= 2, "conv3x3_tc: axis must be 0, 1 or 2 (got %d)", c.axis);
-  if (d.res_w || d.add) return set_err(B200_ERR_UNSUPPORTED, "conv3x3_tc: the folded residual and the epilogue add are 3x3x3 forms only");
+  if (d.res_w) return set_err(B200_ERR_UNSUPPORTED, "conv3x3_tc: the folded residual is a 3x3x3 form only");
   return conv_tc_dispatch(d, c);
 }
 

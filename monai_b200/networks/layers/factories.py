@@ -41,13 +41,15 @@ def get_norm_layer(name, spatial_dims: int = 1, channels: int | None = 1):
         return nn.Identity()
     norm_name, kw = split_args(name)
     key = str(norm_name).lower()
-    if key == "instance":
+    # "instance_nvfuser" is apex's InstanceNorm3dNVFuser; the reference's factory falls back to nn.InstanceNorm{1,2,3}d without apex
+    # (monai/networks/layers/factories.py:258-281), the same arithmetic
+    if key in ("instance", "instance_nvfuser"):
         return (nn.InstanceNorm1d, nn.InstanceNorm2d, nn.InstanceNorm3d)[spatial_dims - 1](channels, **kw)
     if key == "batch":
         return (nn.BatchNorm1d, nn.BatchNorm2d, nn.BatchNorm3d)[spatial_dims - 1](channels, **kw)
     if key == "group":   # Norm.GROUP (monai/networks/layers/factories.py): nn.GroupNorm(num_groups, num_channels, ...)
         return nn.GroupNorm(num_channels=channels, **kw)
-    raise NotImplementedError(f"monai_b200 supports 'instance', 'batch' and 'group' normalisation, got {norm_name!r}.")
+    raise NotImplementedError(f"monai_b200 supports 'instance', 'instance_nvfuser', 'batch' and 'group' normalisation, got {norm_name!r}.")
 
 
 def get_dropout_layer(name, dropout_dim: int = 1):

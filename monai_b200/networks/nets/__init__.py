@@ -3,5 +3,6 @@ from .unet import UNet, Unet
 from .swin_unetr import SwinUNETR
 from .dynunet import DynUNet, DynUnet, Dynunet
 from .segresnet import SegResNet
+from .segresnet_ds import SegResNetDS
 from .unetr import UNETR
 from .vit import ViT

@@ -1,4 +1,5 @@
-"""`TcNet`: the mixin every network with a tensor-core forward (UNet, BasicUNet, SwinUNETR, UNETR, DynUNet, SegResNet) inherits.
+"""`TcNet`: the mixin every network with a tensor-core forward (UNet, BasicUNet, SwinUNETR, UNETR, DynUNet, SegResNet, SegResNetDS)
+inherits.
 
 It owns what those networks share:
   * `forward`: the choice between `_forward_tc` (fp16 channel-blocked "NC8" buffers on Hopper tensor cores) and `_forward_generic`

@@ -16,11 +16,16 @@
                          eval-mode BatchNorm, PReLU, 1 -> 2 channels); a 256^3 fp16 volume, roi 160^3;
   * unet res_instance:   the same net with InstanceNorm (MONAI's default norm); a 256^3 fp16 volume, roi 96^3;
   * basic_unet:          the reference's defaults (features 32, 32, 64, 128, 256, 32, affine instance norm, LeakyReLU 0.1, 1 -> 2
-                         channels); a 256^3 fp16 volume, roi 96^3.
+                         channels); a 256^3 fp16 volume, roi 96^3;
+  * segresnet_ds default:  the reference's defaults (init 32, eval-mode BatchNorm, ReLU, deconv, blocks (1,2,2,4), 1 -> 2 channels);
+                         a 256^3 fp16 volume, roi 96^3;
+  * segresnet_ds auto3dseg: the net of MONAI's Auto3DSeg `segresnet` algorithm on thick-slice CT (init 32, blocks (1,2,2,4,4),
+                         instance norm, resolution (0.8, 0.8, 2.5): [3,3,1] kernels and (2,2,1) strides at level 0, 1 -> 14
+                         channels); a 512 x 512 x 128 fp16 volume, roi 192 x 192 x 64.
 
-    python scripts/sliding_window_tc.py --net unetr|dynunet|segresnet|unet|basic_unet [--workload brats|wholebody|both (SegResNet) |
-                                        iso|aniso_d|aniso_w|all (DynUNet) | res_batch|res_instance|res (UNet)] [--sw-batch 4]
-                                        [--steps 3] [--warmup 1]
+    python scripts/sliding_window_tc.py --net unetr|dynunet|segresnet|unet|basic_unet|segresnet_ds [--workload brats|wholebody|both
+                                        (SegResNet) | iso|aniso_d|aniso_w|all (DynUNet) | res_batch|res_instance|res (UNet) |
+                                        default|auto3dseg|ds (SegResNetDS)] [--sw-batch 4] [--steps 3] [--warmup 1]
 
 Overlap 0.5, gaussian blending.  Every batch shape (the full batches and the remainder batch) is warmed up first; each timed step
 is bracketed by CUDA events with a 256 MiB L2 flush before it (outside the timed interval), and the spread of the timed steps is
@@ -183,6 +188,36 @@ def basic_unet_flops(net, roi) -> dict:
     return {"encoder": enc, "decoder": dec, "total": enc + dec}
 
 
+def segresnet_ds_flops(net, roi) -> dict:
+    """Multiply-add FLOPs (x2) of one window, from the module shapes of SegResNetDS: conv_init, both convolutions of every
+    SegResBlock and the strided convolutions (encoder); the transposed convolutions or 1x1 preconvs, the up blocks and the head
+    (decoder).  A transposed convolution costs every tap per input voxel."""
+    scales = net.anisotropic_scales or [(2, 2, 2)] * len(net.blocks_down)
+    sp = [tuple(roi)]
+    for sc in scales[: len(net.blocks_down) - 1]:
+        sp.append(tuple(s // int(f) for s, f in zip(sp[-1], sc)))
+    v = [math.prod(s) for s in sp]                                   # voxels at level k
+
+    def conv(n, m):
+        return 2.0 * n * m.in_channels * m.out_channels * math.prod(m.kernel_size)
+
+    def blocks(seq, n):
+        return sum(conv(n, b.conv1) + conv(n, b.conv2) for b in seq)
+
+    enc = conv(v[0], net.encoder.conv_init)
+    for k, lvl in enumerate(net.encoder.layers):
+        enc += blocks(lvl["blocks"], v[k])
+        if k + 1 < len(v):
+            enc += conv(v[k + 1], lvl["downsample"])               # output voxels
+    dec, n_up = 0.0, len(net.blocks_down) - 1
+    for i, lvl in enumerate(net.up_layers[:n_up]):
+        k, up = n_up - 1 - i, lvl["upsample"]                      # the level the decoder step lands on
+        dec += conv(v[k + 1], up.deconv if hasattr(up, "deconv") else up.preconv)
+        dec += blocks(lvl["blocks"], v[k])
+    dec += conv(v[0], net.up_layers[-1]["head"])
+    return {"encoder": enc, "decoder": dec, "total": enc + dec}
+
+
 def unet_act_passes(net, roi, batch) -> list:
     """(channels, spatial size) of each activation-only norm_act_nc8 pass of a BatchNorm residual UNet forward: the output of every
     unit of a down or bottom ResidualUnit but its last, activated before the next unit's convolution reads it."""
@@ -199,7 +234,7 @@ def unet_act_passes(net, roi, batch) -> list:
 
 
 def _nets():
-    from monai_b200.networks.nets import UNETR, BasicUNet, DynUNet, SegResNet, UNet
+    from monai_b200.networks.nets import UNETR, BasicUNet, DynUNet, SegResNet, SegResNetDS, UNet
 
     return {
         "unetr": {
@@ -243,6 +278,16 @@ def _nets():
             "basic_unet_sliding_window": dict(
                 make=lambda: BasicUNet(), seed=70, cin=1, volume=(256, 256, 256), roi=(96, 96, 96), flops=basic_unet_flops, eager_vs_replay=True,
                 desc="BasicUNet(in=1, out=2, features (32, 32, 64, 128, 256, 32), affine IN, LeakyReLU 0.1)"),
+        },
+        "segresnet_ds": {
+            "segresnet_ds_sliding_window_default": dict(
+                make=lambda: SegResNetDS(), seed=110, cin=1, volume=(256, 256, 256), roi=(96, 96, 96), flops=segresnet_ds_flops,
+                desc="SegResNetDS(init=32, in=1, out=2, BatchNorm (eval), ReLU, blocks (1, 2, 2, 4), deconv)"),
+            "segresnet_ds_sliding_window_auto3dseg": dict(
+                make=lambda: SegResNetDS(init_filters=32, in_channels=1, out_channels=14, blocks_down=(1, 2, 2, 4, 4), norm="instance_nvfuser",
+                                         dsdepth=4, resolution=(0.8, 0.8, 2.5)),
+                seed=111, cin=1, volume=(512, 512, 128), roi=(192, 192, 64), flops=segresnet_ds_flops,
+                desc="SegResNetDS(init=32, in=1, out=14, instance norm, blocks (1, 2, 2, 4, 4), dsdepth 4, resolution (0.8, 0.8, 2.5), deconv)"),
         },
     }
 
@@ -373,11 +418,11 @@ def run(metric: str, wl: dict, args, card: dict) -> dict:
 
 def main() -> None:
     ap = argparse.ArgumentParser()
-    ap.add_argument("--net", required=True, choices=["unetr", "dynunet", "segresnet", "unet", "basic_unet"])
+    ap.add_argument("--net", required=True, choices=["unetr", "dynunet", "segresnet", "unet", "basic_unet", "segresnet_ds"])
     ap.add_argument("--workload", default=None, choices=["both", "brats", "wholebody", "all", "iso", "aniso_d", "aniso_w", "res_batch",
-                                                          "res_instance", "res"],
+                                                          "res_instance", "res", "default", "auto3dseg", "ds"],
                     help="SegResNet: brats|wholebody|both (default both); DynUNet: iso|aniso_d|aniso_w|all (default iso); "
-                         "UNet: res_batch|res_instance|res (default res: both)")
+                         "UNet: res_batch|res_instance|res (default res: both); SegResNetDS: default|auto3dseg|ds (default ds: both)")
     ap.add_argument("--sw-batch", type=int, default=4)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
@@ -393,6 +438,8 @@ def main() -> None:
         workloads = {name: workloads[name]}
     if args.net == "unet" and args.workload not in (None, "res"):
         workloads = {f"unet_sliding_window_{args.workload}": workloads[f"unet_sliding_window_{args.workload}"]}
+    if args.net == "segresnet_ds" and args.workload not in (None, "ds"):
+        workloads = {f"segresnet_ds_sliding_window_{args.workload}": workloads[f"segresnet_ds_sliding_window_{args.workload}"]}
     card = _card()
     for metric, wl in workloads.items():
         print(json.dumps(run(metric, wl, args, card)), flush=True)
